@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — frames/s through detect -> match -> local BA at 1920x1080 mono (BASELINE.json metric), one JSON line.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A step is one frame through the whole hot path: ORB extract (2000 kp) of a NEW 1080p frame, 256-bit Hamming match against the
 previous frame's descriptors, and one local bundle adjustment (50 keyframes / 2000 landmarks / 10 000 observations, 10 LM
@@ -18,14 +18,15 @@ iterations, 50-iteration block-Jacobi PCG cap).
                all-reduce of the compact reduced camera system per LM iteration -- STRONG scaling (total work fixed).
 N>1 for the per-frame path: independent replicas, one rank per GPU, no data-path collective -> weak scaling.
 
-The timed block of K steps is repeated (each repetition bracketed by barrier + synchronize, max over ranks) and the MEDIAN block is
-reported, so that a 20-step run is not a 24 ms coin flip; the clock sampler starts before the warm-up.
+`value` times exactly K steps after W warm-up steps, in one window bracketed by barrier + synchronize (max over ranks); the clock
+sampler starts before the warm-up.  --dump-outputs DIR writes what the last timed step computed (keypoints, descriptors, matches,
+the solved window and its LM result) as DIR/<name>.npy; the inputs depend only on the arguments, so two builds can be compared.
+The secondary sections bound their own step counts and report them: config4_stereo runs 10..50 steps, e2e 10..100.
 """
 from __future__ import annotations
 
 import argparse
 import json
-import math
 import os
 import queue
 import subprocess
@@ -40,7 +41,7 @@ sys.path.insert(0, ROOT)
 
 W, H, NKP = 1920, 1080, 2000
 BA_CAMS, BA_PTS, BA_OBS_PER_PT, BA_ITERS, PCG_ITERS = 50, 2000, 5, 10, 50
-RING = 72  # frames resident in HBM: 72 * 2.07 MB = 149 MB > 126 MB L2
+RING = 72  # frames resident in HBM: 72 * 2.07 MB = 149 MB, about three times the 50 MB L2 of an H100
 GBA_CAMS, GBA_PTS, GBA_OBS_PER_PT, GBA_ITERS, GBA_PCG = 500, 100000, 10, 5, 30
 METRIC = "frames/sec detect+match+local-BA @1920x1080 mono"
 
@@ -69,7 +70,7 @@ def workload_config(world):
     """The `config` object: identical keys in both arms (the driver compares them)."""
     return {"workload": (f"{W}x{H} mono, {NKP} kp ORB extract + {NKP}x{NKP} Hamming match + local BA "
                          f"({BA_CAMS} KF/{BA_PTS} pts/{BA_PTS * BA_OBS_PER_PT} obs, {BA_ITERS} LM it, PCG cap {PCG_ITERS})"),
-            "l2": f"input ring of {RING} frames ({RING * W * H / 1e6:.0f} MB) > 126 MB L2",
+            "l2": f"input ring of {RING} frames ({RING * W * H / 1e6:.0f} MB) > 50 MB L2",
             "parallelism": f"replicas x{world}; tracking (extract+match) and mapping (local BA) pipelined"}
 
 
@@ -175,6 +176,22 @@ def cpu_path(frames, ba_problem, steps, threads):
     return steps / dt, what
 
 
+def dump_outputs(out_dir, feats, graph, res):
+    """What a caller of the timed step receives for its last frame: the frame's keypoints and descriptors, its matches against
+    the previous frame, and the solved BA window with its LM result."""
+    os.makedirs(out_dir, exist_ok=True)
+    kps, desc = feats.download()
+    idx, d1, d2 = feats.matches()
+    poses, points = graph.download()
+    arrays = {"keypoints": np.stack([kps[f].astype(np.float32) for f in kps.dtype.names], axis=1).reshape(-1, len(kps.dtype.names)),
+              "descriptors": desc.astype(np.float32),
+              "match_index": idx.astype(np.float32), "match_distance": d1.astype(np.float32), "match_distance2": d2.astype(np.float32),
+              "ba_poses_wc": poses.astype(np.float64), "ba_points": points.astype(np.float64),
+              "ba_result": np.array([res.initial_cost, res.final_cost, res.iterations, res.accepted, res.pcg_iterations], np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def median(xs):
     return float(np.median(np.asarray(xs, dtype=np.float64)))
 
@@ -186,7 +203,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--no-global-ba", action="store_true", help="skip the config-5 global BA section")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be at least 1 and --warmup at least 0")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of the device path; it does not apply to --impl reference")
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
     from gslam_b200 import synth
     ba_problem = synth.synth_ba(BA_CAMS, BA_PTS, BA_OBS_PER_PT, seed=42, n_fixed=2)
@@ -195,17 +217,17 @@ def main():
     if args.impl == "reference":
         if rank != 0:
             return
-        steps = max(1, min(args.steps, 20))
-        warm = max(1, min(args.warmup, 3))
+        steps = args.steps
         frames = synth.synth_stream(W, H, 4, seed=7)
-        cpu_path(frames, ba_problem, warm, cores)
+        if args.warmup > 0:
+            cpu_path(frames, ba_problem, args.warmup, cores)
         fps, what = cpu_path(frames, ba_problem, steps, cores)
         line = {"impl": "reference", "metric": METRIC, "value": fps, "unit": "frames/s",
                 "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 / fps,
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8+f64", "data": "synthetic",
                 "config": workload_config(world),
                 "cpu_baseline": {"value": fps, "unit": "frames/s", "cores": cores, "kind": "port",
-                                 "sample": f"{steps} frames after {warm} warm-up (bounded sample of the --steps/--warmup asked): {what}"},
+                                 "sample": f"{steps} frames after {args.warmup} warm-up: {what}"},
                 "e2e": {"value": fps, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
         print(json.dumps(line))
         return
@@ -258,6 +280,8 @@ def main():
         for k in range(k0, k0 + n):
             step_serial(k)
 
+    last_ba = [None]
+
     def run_pipelined(k0, n):
         """n frames from two host threads, like a SLAM's tracking and mapping threads: the tracking thread enqueues extract(k) +
         match(k) (no host synchronisation: the matcher reads the keypoint counts on the device) and orders the mapping stream
@@ -272,7 +296,7 @@ def main():
                     if k is None:
                         return
                     graph_p.reset()
-                    graph_p.solve(ba_cfg)
+                    last_ba[0] = graph_p.solve(ba_cfg)
             except Exception as e:
                 err.append(e)
         th = threading.Thread(target=mapper, daemon=True)
@@ -287,37 +311,30 @@ def main():
             raise err[0]
         ctx.wait_for(ctx_m)              # the timing events live on the tracking stream
 
-    def timed_blocks(run, steps):
-        """Repeat [barrier, K steps, barrier] and return the per-block ms (max over ranks each) and the launch count of a block."""
-        blocks, out, launches = None, [], 0
-        k0 = args.warmup
-        b = 0
-        while True:
-            barrier()
-            l0 = ctx.launch_count() + ctx_m.launch_count()
-            ctx.timer_begin()
-            run(k0, steps)
-            ms = ctx.timer_end()
-            torch.cuda.synchronize()
-            launches = ctx.launch_count() + ctx_m.launch_count() - l0
-            out.append(max_over_ranks(ms))
-            k0 += steps
-            b += 1
-            if blocks is None:  # enough repetitions for >= ~0.7 s of timed work and at least 5 blocks (every rank agrees: max'd time)
-                blocks = int(min(60, max(5, math.ceil(700.0 / max(out[0], 1e-3)))))
-            if b >= blocks:
-                return out, launches
+    def timed(run, steps):
+        """[barrier, steps steps from frame --warmup on, barrier]: the ms (max over ranks) and the launch count of the window."""
+        barrier()
+        l0 = ctx.launch_count() + ctx_m.launch_count()
+        ctx.timer_begin()
+        run(args.warmup, steps)
+        ms = ctx.timer_end()
+        torch.cuda.synchronize()
+        return max_over_ranks(ms), ctx.launch_count() + ctx_m.launch_count() - l0
 
     feats[1].extract(ring[RING - 1].data_ptr(), W, H, cfg, device_ptr=True, pitch=W)
-    run_serial(0, max(3, args.warmup))
-    run_pipelined(0, max(3, args.warmup))
+    run_serial(0, args.warmup)
+    run_pipelined(0, args.warmup)
     ctx.sync(); ctx_m.sync()
     if sampler:
         sampler.mark()
-    ser_ms, ser_launches = timed_blocks(run_serial, args.steps)
-    pip_ms, pip_launches = timed_blocks(run_pipelined, args.steps)
+    ms_serial, ser_launches = timed(run_serial, args.steps)
+    # the first step of the window matches against the frame before it, whatever --steps the serial window ran
+    feats[(args.warmup + 1) & 1].extract(ring[(args.warmup - 1) % RING].data_ptr(), W, H, cfg, device_ptr=True, pitch=W)
+    ctx.sync()
+    ms_pipe, pip_launches = timed(run_pipelined, args.steps)
     clocks = sampler.finish() if sampler else None
-    ms_serial, ms_pipe = median(ser_ms), median(pip_ms)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, feats[(args.warmup + args.steps - 1) & 1], graph_p, last_ba[0])
 
     # ---- per-stage device timing (CUDA events on the ctx stream) ------------------------------------------------------------
     def time_stage(fn, reps, c=ctx):
@@ -562,25 +579,19 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         peak, peak_src = float(peaks["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
     except Exception:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "NVIDIA H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
     def gbs(nbytes, ms_):
         return nbytes / (ms_ * 1e-3) / 1e9
     ach = gbs(big_bytes, t_sweep_big)
-    traffic = None
-    try:  # per-launch DRAM bytes of the sweep from the committed ncu capture of this round (profiles/r02_sweep_traffic.json)
-        traffic = float(json.load(open(os.path.join(ROOT, "profiles", "r02_sweep_traffic.json")))["dram_bytes_per_launch"])
-        traffic_src = "profiles/r02_sweep_traffic.json (dram__bytes_read.sum + dram__bytes_write.sum of one launch, ncu --set full)"
-    except Exception:
-        traffic, traffic_src = 150.6e6, "profiles/r01_ncu_summary.md (44.25 MB read + 106.36 MB written, one launch, ncu --set full; round-1 kernel)"
     line = {"metric": METRIC, "value": fps, "unit": "frames/s", "n_gpus": world,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_pipe / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "u8+f64", "data": "synthetic",
             "config": workload_config(world),
-            "timing": {"blocks": len(pip_ms), "block_ms_median": ms_pipe, "block_ms_min": min(pip_ms), "block_ms_max": max(pip_ms),
-                       "rule": "each block = exactly --steps steps between barrier+synchronize, CUDA events, max over ranks; median block reported"},
-            "serial": {"value": world * args.steps / (ms_serial * 1e-3), "ms_per_step": ms_serial / args.steps, "blocks": len(ser_ms),
-                       "note": "the same steps on ONE stream (round-1 definition of `value`)", "gpu_launches": int(ser_launches)},
+            "timing": {"window_ms": ms_pipe,
+                       "rule": "exactly --steps steps after --warmup warm-up steps between barrier+synchronize, CUDA events, max over ranks"},
+            "serial": {"value": world * args.steps / (ms_serial * 1e-3), "ms_per_step": ms_serial / args.steps,
+                       "note": "the same steps on ONE stream", "gpu_launches": int(ser_launches)},
             "clocks": clocks, "gpu_launches": int(pip_launches),
             "e2e": {"value": e2e_pipe_pageable, "unit": "frames/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                     "steps": e2e_steps, "host_memory": "pageable (malloc'd like GImage); tracking thread || mapping thread, two gb_ctx",
@@ -593,8 +604,6 @@ def main():
             # dominant HBM-bound kernel of the path = the BA Jacobian sweep (BASELINE metric, 2nd clause), at config-5 size
             "roofline": {"kernel": "BA Jacobian sweep K6 (ba_sweep_kernel: camera items + landmark items in one persistent launch), 500 cams/100k pts/1M obs",
                          "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                         "traffic": traffic, "traffic_source": traffic_src,
-                         "frac_on_measured_dram_bytes": (traffic / (t_sweep_big * 1e-3) / 1e9) / peak if traffic else None,
                          "in_timed_step": False,
                          "peak_source": peak_src, "algorithmic_bytes": int(big_bytes), "ms_per_sweep": t_sweep_big},
             # the same quantity for the kernels as they run inside the timed step (one frame / one 10k-observation window:

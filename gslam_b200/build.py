@@ -1,8 +1,7 @@
-"""In-tree build of the sm_100a CUDA library and the reference-facing C++ plugins.
+"""In-tree build of the sm_90a (H100) CUDA library.
 
-`python -m gslam_b200.build` (or __graft_entry__.build()) cross-compiles with nvcc for sm_100a — no GPU needed — into
-gslam_b200/lib/.  The .so files are git-ignored but travel to the GPU box with the gpurun snapshot; a content hash
-(.stamp) decides whether a rebuild is needed, so the box never rebuilds an up-to-date library.
+`python -m gslam_b200.build` (or __graft_entry__.build()) cross-compiles with nvcc for sm_90a — no GPU needed — into
+gslam_b200/lib/.  The .so files are git-ignored; a content hash (.stamp) decides whether a rebuild is needed.
 """
 from __future__ import annotations
 
@@ -16,13 +15,10 @@ import sys
 ROOT = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(ROOT)
 CSRC = os.path.join(ROOT, "csrc")
-PLUGIN = os.path.join(ROOT, "plugin")
 LIBDIR = os.path.join(ROOT, "lib")
 OBJDIR = os.path.join(ROOT, "build")
 KERNEL_LIB = os.path.join(LIBDIR, "libgslam_b200_kernels.so")
-REFERENCE = "/root/reference"
-
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -79,7 +75,7 @@ def build_kernels(force: bool = False, verbose: bool = False) -> str:
 
     with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, len(cu))) as ex:
         objs = list(ex.map(compile_one, cu))
-    cmd = [nvcc, "-shared", "-o", KERNEL_LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", KERNEL_LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
@@ -88,30 +84,8 @@ def build_kernels(force: bool = False, verbose: bool = False) -> str:
     return KERNEL_LIB
 
 
-def build_plugins(force: bool = False) -> list[str]:
-    """The GSLAM-facing C++ shims need the reference headers: built where /root/reference exists, shipped prebuilt."""
-    if not os.path.isdir(PLUGIN):
-        return []
-    srcs = sorted(os.path.join(PLUGIN, f) for f in os.listdir(PLUGIN) if f.endswith((".cpp", ".h", ".mk")) or f == "Makefile")
-    if not os.path.exists(os.path.join(PLUGIN, "Makefile")):
-        return []
-    stamp_path = os.path.join(LIBDIR, ".stamp_plugins")
-    want = _hash(srcs + [os.path.join(REPO, "include", "gslam_b200.h")])
-    outs = [os.path.join(LIBDIR, n) for n in ("libgslam_optimizer.so", "libgslam_b200.so", "libgslam_estimator.so", "libgslamDB_synth.so", "gslam_b200_host_test")]
-    if not force and all(os.path.exists(o) for o in outs) and os.path.exists(stamp_path) and open(stamp_path).read() == want:
-        return outs
-    if not os.path.isdir(os.path.join(REFERENCE, "GSLAM", "core")):
-        return [o for o in outs if os.path.exists(o)]  # GPU box: use the prebuilt files
-    os.makedirs(LIBDIR, exist_ok=True)
-    subprocess.check_call(["make", "-C", PLUGIN, "-s", f"REF={REFERENCE}", f"LIBDIR={LIBDIR}"])
-    with open(stamp_path, "w") as f:
-        f.write(want)
-    return outs
-
-
 def build_all(force: bool = False, verbose: bool = False) -> None:
     build_kernels(force, verbose)
-    build_plugins(force)
 
 
 if __name__ == "__main__":

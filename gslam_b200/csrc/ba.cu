@@ -474,8 +474,7 @@ __global__ void __launch_bounds__(128) ba_schur_blocks_kernel(BaDev g, double* _
 constexpr int kChunkCams = 16, kChunkSlots = kChunkCams * (kChunkCams + 1) / 2, kChunkThreads = 160, kChunkBatch = 4;
 constexpr int kChunkMaxLm = 64;  // landmarks per chunk (host plan)
 
-// v4 (profiles/r02_ncu_summary.md: v3 issued 958 warp-instructions per landmark at 10 warps / SM -- index arithmetic of the
-// staging loops, idle lanes, DMUL+DADD around the DFMAs):
+// v4 (v3 spent its issue slots on index arithmetic of the staging loops, idle lanes and DMUL+DADD around the DFMAs):
 //  * the W blocks of a batch are staged EDGE-indexed: a landmark's blocks are contiguous in global memory, so staging is a plain
 //    16-byte-granular copy; the slot threads find their two edges with one popcount each;
 //  * thread t works the t-th slot the chunk really uses (host table), so a chunk over 10 cameras keeps exactly 55 lanes busy;
@@ -483,7 +482,7 @@ constexpr int kChunkMaxLm = 64;  // landmarks per chunk (host plan)
 //    blocks in flight (cp.async) during the arithmetic;
 //  * acc = fma(y0, w0, fma(y1, w1, fma(y2, w2, acc))): 108 DFMA per (landmark, slot), nothing else on the fp64 pipe.
 //  * v6: TWO threads per slot (rows 0-2 / rows 3-5 of the 6x6 block): v5 kept 2 of a CTA's 5 warps busy in the accumulation and the
-//    fp64 pipe 18 % active (profiles/r02_ncu_summary.md); halving the per-thread accumulator also frees registers for 4 CTAs / SM.
+//    fp64 pipe mostly idle; halving the per-thread accumulator also frees registers for 4 CTAs / SM.
 //    A chunk with more than 80 used slots (13+ cameras; the planner avoids it) is worked in passes of 80 slots.
 constexpr int kChunkSlotsPerPass = kChunkThreads / 2;
 

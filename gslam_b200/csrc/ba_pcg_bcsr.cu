@@ -4,8 +4,8 @@
 // CPU checker (oracle/ba_ref.c::ba_pcg) and as the generic multi-kernel path it replaces (ba.cu: pcg_matvec / pcg_update).
 //
 // Why: at BASELINE config 5 (500 cameras / 100k landmarks / 1M observations) the dense S is 72 MB and one PCG iteration of the
-// generic path is two launches that re-read it from HBM; the covisibility fill is ~20 %, so block-CSR S is ~14 MB -- 97 KB per SM
-// when the block rows are dealt out over the 148 SMs, i.e. it FITS IN SHARED MEMORY for the whole solve.  What remains per
+// generic path is two launches that re-read it from HBM; the covisibility fill is ~20 %, so block-CSR S is ~14 MB -- 109 KB per SM
+// when the block rows are dealt out over the 132 SMs, i.e. it FITS IN SHARED MEMORY for the whole solve.  What remains per
 // iteration is latency: two grid barriers (the inner products; the publication of u = M^-1 r), a 24 KB read of u from L2 and
 // ~12 k DFMA per CTA.  The same kernel runs replicated and bit-identically on every rank of the landmark-sharded solve (the
 // all-reduced compact system is its input), so the ranks take identical LM decisions without any broadcast.
@@ -60,7 +60,7 @@ __device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int& ta
 
 // CLUSTER = true: the whole grid is ONE thread-block cluster (<= 16 CTAs, chosen on the host when S fits their shared memory):
 // u and the per-CTA (gamma, delta) partials travel through distributed shared memory and the two barriers per iteration are
-// hardware cluster barriers (~0.2 us) instead of a global-memory ticket barrier (~1-1.5 us with 148 CTAs).
+// hardware cluster barriers (~0.2 us) instead of a global-memory ticket barrier (one CTA per SM).
 template <bool CLUSTER>
 __global__ void __launch_bounds__(kBcsrThreads, 1) ba_pcg_bcsr_kernel(BaDev g, double* __restrict__ rbuf, BcsrArgs a) {
   namespace cg = cooperative_groups;

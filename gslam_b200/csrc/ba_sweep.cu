@@ -384,7 +384,7 @@ __global__ void __launch_bounds__(kSwThreads, 1) ba_sweep_kernel(BaDev g, int wh
 
 // Host plan.  Landmark groups: consecutive landmarks with <= 128 observations and <= 32 landmarks together (a landmark with more
 // observations than a chunk is a group of its own, swept in several chunks).  Camera slices as ba.cu cuts them.  The items are dealt
-// to n_teams teams so that every team carries about the same cost (cost model measured on a B200: a camera-pass observation is
+// to n_teams teams so that every team carries about the same cost (cost model: a camera-pass observation is
 // 0.4 of a landmark-pass observation, plus a fixed fold per camera slice): team k gets camera slices k, k + n_teams, ... and then a
 // CONTIGUOUS run of landmark groups (neighbouring groups share pose-table and landmark cache lines).
 void ba_sweep_plan_host(int nc, int np, int cam_split, const std::vector<int>& cam_off, const std::vector<int>& pt_off, int n_teams,

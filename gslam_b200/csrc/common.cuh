@@ -1,4 +1,4 @@
-// gslam_b200/csrc/common.cuh — context, error plumbing and small device helpers shared by the sm_100a kernels.
+// gslam_b200/csrc/common.cuh — context, error plumbing and small device helpers shared by the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -17,7 +17,7 @@ struct MatchState;  // match.cu
 
 struct gb_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int max_smem_optin = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // gb_timer_*

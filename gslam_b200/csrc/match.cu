@@ -6,7 +6,7 @@
 // Shape of the work: Q x T pairs, each 8 XOR + 8 POPC + adds on 32-byte rows.  Algorithmic HBM traffic is only
 // 32(Q+T)+12Q bytes, so this kernel is bound by the integer POPC pipe, not by HBM (DESIGN.md §match).  One thread owns
 // one query row in registers; a CTA stages a chunk of train rows in shared memory and every lane reads the same row
-// (broadcast, conflict-free).  The train dimension is split across blockIdx.y so that Q=2000 still fills 148 SMs; the
+// (broadcast, conflict-free).  The train dimension is split across blockIdx.y so that Q=2000 still fills 132 SMs; the
 // last CTA of each query tile (atomic ticket) merges the per-chunk (best, 2nd) partials in ascending chunk order, which
 // reproduces the sequential "first minimum wins" tie rule exactly.  One launch, no atomics on the data path.
 #include "common.cuh"

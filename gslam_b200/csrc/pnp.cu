@@ -1,9 +1,7 @@
 // gslam_b200/csrc/pnp.cu — P3P + RANSAC pose estimation from 3D-2D matches: the kernel side of SURVEY.md §8f-1,
 // GSLAM::Estimator::findPnP (GSLAM/core/Estimator.h:158-164; factory :175-191).
 //
-// STATUS: written at the end of round 1 after the GPU budget was spent — it compiles for sm_100a and mirrors the CPU checker
-// operation for operation, but it has NOT run on a B200 yet (tools/gpu_pnp_check.py is the first thing to run; no test under
-// tests/ exercises it until then).
+// It mirrors the CPU checker operation for operation; tests/test_pnp_gpu.py compares the two.
 //
 // Design: RANSAC hypotheses are independent work items.  Hypothesis h draws its three correspondences from a counter-based
 // generator (splitmix64 of seed and h: no sequential state), solves P3P (Grunert's distance formulation: quartic in v = s3/s1 built

@@ -1,9 +1,9 @@
 // gslam_b200/plugin/estimator_b200.cpp -> libgslam_estimator.so
 //
-// A GSLAM::Estimator (GSLAM/core/Estimator.h:93-193) whose findPnP() runs P3P + RANSAC + refinement on the B200 through
+// A GSLAM::Estimator (GSLAM/core/Estimator.h:93-193) whose findPnP() runs P3P + RANSAC + refinement on the GPU through
 // gb_pnp_ransac (include/gslam_b200.h).  Found by GSLAM::Estimator::create() like the (absent) default estimator plugin:
 // Registry::get(svar "EstimatorPlugin" = "libgslam_estimator") -> dlsym("createEstimatorInstance") (Estimator.h:175-191, 43-45).
-// SURVEY.md §8f-1.  STATUS: compiles and links; the kernel behind it has not run on a B200 yet (see csrc/pnp.cu).
+// SURVEY.md §8f-1.
 //
 // Contract kept from the reference: bool returns, never throws across the boundary, `const` methods, the optional mask receives one
 // byte per correspondence.  Only findPnP is implemented; every other model returns false (the reference's own convention for an

@@ -1,7 +1,7 @@
 // gslam_b200/plugin/host_test.cpp -> gslam_b200_host_test
 //
 // A stand-in for a GSLAM SLAM plugin: it uses ONLY the reference's public API (Optimizer::create, Registry::load, Svar calls,
-// BundleGraph, GImage, KeyPoint) to drive the B200 backends, reading a case from a binary file and writing the results back,
+// BundleGraph, GImage, KeyPoint) to drive the GPU backends, reading a case from a binary file and writing the results back,
 // so the Python tests can compare the plugin-level outputs with the oracle.  Usage:
 //   gslam_b200_host_test ba   <plugin-dir> in.bin out.bin      optimize(BundleGraph&) through GSLAM::Optimizer::create()
 //   gslam_b200_host_test pnp  <plugin-dir> in.bin out.bin      optimizePnP(...)

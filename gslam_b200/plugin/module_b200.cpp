@@ -173,7 +173,7 @@ class B200Vocabulary : public GSLAM::Vocabulary {
 
 // ---- the Messenger-level application (SURVEY.md section 8f-2) ---------------------------------------------------------------------
 // `gslam play b200_features [metric_time -slam b200] -dataset x.synth`: subscribes "dataset/frame" (published by the reference's
-// player, GSLAM/plugins/play/main.cpp:15,126-132), runs the B200 feature path on every frame -- ORB extract on each camera of the
+// player, GSLAM/plugins/play/main.cpp:15,126-132), runs the GPU feature path on every frame -- ORB extract on each camera of the
 // frame, MapFrame::setKeyPoints (Map.h:311), Hamming match against the previous frame, row-band stereo match for two-camera frames
 // -- and publishes the frame on "<name>/curframe", the topic GSLAM's own latency tool listens to
 // (GSLAM/evaluation/metric_time/main.cpp:11-21), plus the associations on "<name>/matches".

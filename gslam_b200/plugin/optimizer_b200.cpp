@@ -1,6 +1,6 @@
 // gslam_b200/plugin/optimizer_b200.cpp -> libgslam_optimizer.so
 //
-// The drop-in: a GSLAM::Optimizer (GSLAM/core/Optimizer.h:184-253) whose optimize()/optimizePnP() run on the B200 through
+// The drop-in: a GSLAM::Optimizer (GSLAM/core/Optimizer.h:184-253) whose optimize()/optimizePnP() run on the GPU through
 // the C-ABI of include/gslam_b200.h.  Found by GSLAM::Optimizer::create() exactly like the (absent) Ceres plugin:
 // Registry::get("libgslam_optimizer") -> dlsym("createOptimizerInstance") (Optimizer.h:234-248, 42-51).
 // This TU is built with default symbol visibility: GSLAM_REGISTER_OPTIMIZER adds no visibility attribute (SURVEY.md §8b).

@@ -1,5 +1,5 @@
 /*
- * gslam_b200.h — the C-ABI drop-in boundary of the B200 backends for GSLAM's per-frame numeric hot path
+ * gslam_b200.h — the C-ABI drop-in boundary of the H100 (sm_90a) backends for GSLAM's per-frame numeric hot path
  * (ORB extract -> 256-bit Hamming brute-force match -> GSLAM::Optimizer bundle adjustment).
  *
  * Plain C: opaque handles, plain pointers and sizes, `int` status returns, caller-owned output buffers.  No STL, no
@@ -327,8 +327,7 @@ GB_API int gb_ba_graph_finish(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* result)
  * Pose from 3D-2D matches with outliers: minimal P3P solver + RANSAC + non-linear refinement.
  * Sits behind GSLAM::Estimator::findPnP(SE3* world2camera, objectPoints, imagePoints, method = P3_ITERATIVE&RANSAC,
  * threshold = 0.01, confidence = 0.99, mask)  GSLAM/core/Estimator.h:158-164 (factory createEstimatorInstance :43-45,175-191);
- * SURVEY.md section 8f-1.  STATUS: compiled for sm_100a, mirrors the CPU checker operation for operation, NOT yet validated on a
- * B200 (round 2 starts with tools/gpu_pnp_check.py).
+ * SURVEY.md section 8f-1.  Mirrors the CPU checker operation for operation (tests/test_pnp_gpu.py).
  *   xyz: n x 3 world points; xy: n x 2 normalised image points (x/z, y/z);
  *   threshold: inlier bound on the normalised reprojection error; confidence in (0,1); max_hypotheses >= 1; seed: any;
  *   pose_cw: 7 doubles OUT, world->camera as the reference signature asks, layout {qx,qy,qz,qw,tx,ty,tz};

@@ -9,6 +9,12 @@ import subprocess
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
+# a checkout of the GSLAM sources (GSLAM_REFERENCE, else the default location below): the reference checkers and the GSLAM plugins
+# compile against its headers into _ref/, which is built where the checkout is and used as built everywhere else
+REFERENCE = os.environ.get("GSLAM_REFERENCE") or "/root/reference"
+# the GSLAM-facing plugins (gslam_b200/plugin) and the host program that drives them through the reference API
+PLUGIN_DIR = os.path.join(_HERE, "_ref", "plugins")
+KERNEL_LIB = os.path.join(os.path.dirname(_HERE), "gslam_b200", "lib", "libgslam_b200_kernels.so")
 _LIB = None
 _REF = None
 
@@ -70,15 +76,26 @@ def default_orb_cfg(**kw) -> OrbCfgC:
 
 
 def build(force: bool = False) -> None:
-    """Compile liboracle.so (always possible) and _ref/libgslam_ref.so (only where /root/reference exists)."""
+    """Compile liboracle.so (always possible) and, where a GSLAM checkout is found (REFERENCE), _ref/libgslam_ref.so and the plugins
+    in _ref/plugins (these link against the CUDA library, so they are built once it is)."""
     srcs = [os.path.join(_HERE, f) for f in ("hamming_ref.c", "ba_ref.c", "orb_ref.c", "pnp_ref.c", "bow_ref.c", "Makefile")]
     lib = os.path.join(_HERE, "liboracle.so")
     if force or not os.path.exists(lib) or any(os.path.getmtime(s) > os.path.getmtime(lib) for s in srcs):
         subprocess.check_call(["make", "-C", _HERE, "-s", "liboracle.so", "CC=gcc"])
     ref = os.path.join(_HERE, "_ref", "libgslam_ref.so")
-    if os.path.isdir("/root/reference/GSLAM/core") and (
-            force or not os.path.exists(ref) or os.path.getmtime(os.path.join(_HERE, "ref_shim.cpp")) > os.path.getmtime(ref)):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "ref", "CXX=g++"])
+    if not os.path.isdir(os.path.join(REFERENCE, "GSLAM", "core")):
+        return
+    if force or not os.path.exists(ref) or os.path.getmtime(os.path.join(_HERE, "ref_shim.cpp")) > os.path.getmtime(ref):
+        subprocess.check_call(["make", "-C", _HERE, "-s", "ref", "CXX=g++", f"REF={REFERENCE}"])
+    if os.path.exists(KERNEL_LIB):
+        subprocess.check_call(["make", "-C", _HERE, "-s", "plugins", "CXX=g++", f"REF={REFERENCE}"])
+
+
+def digest(a) -> str:
+    """SHA-256 of an array's dtype, shape and bytes: stored golden outputs compared exactly without storing them whole."""
+    import hashlib
+    a = np.ascontiguousarray(a)
+    return hashlib.sha256(f"{a.dtype.str}{a.shape}".encode() + a.tobytes()).hexdigest()[:32]
 
 
 def lib() -> C.CDLL:

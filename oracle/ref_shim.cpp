@@ -1,12 +1,12 @@
 // oracle/ref_shim.cpp — NOT a restatement: a thin extern "C" window onto the UNMODIFIED reference headers, compiled from
-// where they lie under /root/reference into oracle/_ref/libgslam_ref.so (recipe: oracle/Makefile, target `ref`).
+// where they lie in the GSLAM checkout named by REF into oracle/_ref/libgslam_ref.so (recipe: oracle/Makefile, target `ref`).
 // TEST INFRASTRUCTURE ONLY.  It pins the parts of the hot path that DO exist in the reference tree:
 //   * Vocabulary::DistanceFactory::hamming32          GSLAM/core/Vocabulary.h:485-491
 //   * SE3 inverse / point transform / product / exp / log   GSLAM/core/SE3.h:100-131,205-287  (pose conventions of BA)
 //   * sizeof / layout of the carrier PODs             Map.h:122-195, Optimizer.h:106-172, SE3.h:337-339, SIM3.h:290-291
 //   * Undistorter::undistort + the remap table of prepareReMap   GSLAM/core/Undistorter.h:120-348 (the frame-undistortion row)
 //   * Vocabulary::create / load / transform (BoW + feature vector)  GSLAM/core/Vocabulary.h:1051-1130,1890-1930,1558-1736 (the BoW row)
-// No reference source is copied into this repository; the .so is git-ignored and travels to the GPU box prebuilt.
+// No reference source is copied into this repository; the .so is git-ignored.
 #include <cstring>
 #include <GSLAM/core/GSLAM.h>
 #include <GSLAM/core/Optimizer.h>

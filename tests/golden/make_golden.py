@@ -1,4 +1,4 @@
-"""Regenerates the committed golden fixtures in tests/golden/ (run HERE, in the build container).
+"""Regenerates the committed golden fixtures in tests/golden/ (oracle/_ref parts need GSLAM_REFERENCE at build time).
 
   python tests/golden/make_golden.py [hamming] [ba] [orb]
 

@@ -1,5 +1,5 @@
 """Generates tests/golden/bow_golden.npz FROM THE REFERENCE ITSELF (oracle/_ref = GSLAM::Vocabulary compiled from the reference
-headers; needs /root/reference at build time): a vocabulary trained by Vocabulary::create (k = 8, L = 3, TF_IDF / L1_NORM) on 60
+headers; needs GSLAM_REFERENCE at build time): a vocabulary trained by Vocabulary::create (k = 8, L = 3, TF_IDF / L1_NORM) on 60
 "images" of 150 clustered 256-bit descriptors, exported as flat arrays, plus the BowVector / FeatureVector the reference's
 Vocabulary::transform (Vocabulary.h:1558-1622) returns for two query sets at levelsup 0 and 2.
 

@@ -34,3 +34,35 @@ def test_gpu_arm_refuses_to_run_without_a_device():
     r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--steps", "1", "--warmup", "1"], capture_output=True, text=True, timeout=600, cwd=ROOT)
     assert r.returncode != 0
     assert not any(l.startswith("{") for l in r.stdout.splitlines())
+
+
+def test_dump_outputs_writes_the_last_step_as_float_arrays(tmp_path):
+    """bench.py --dump-outputs: what a caller of the timed step receives, one float32 / float64 .npy per array, from stand-ins for
+    the device objects (the device path itself is exercised by the GPU runs of bench.py)."""
+    import importlib.util
+    import types
+    import numpy as np
+    from gslam_b200.capi import KP_DTYPE
+    spec = importlib.util.spec_from_file_location("bench_under_test", os.path.join(ROOT, "bench.py"))
+    bench = importlib.util.module_from_spec(spec); spec.loader.exec_module(bench)
+    n, nc, npts = 5, 3, 4
+    kps = np.zeros(n, KP_DTYPE); kps["x"] = np.arange(n); kps["octave"] = 2
+    feats = types.SimpleNamespace(download=lambda: (kps, np.full((n, 32), 7, np.uint8)),
+                                  matches=lambda: (np.arange(n, dtype=np.int32), np.full(n, 3, np.int32), np.full(n, 9, np.int32)))
+    graph = types.SimpleNamespace(download=lambda: (np.ones((nc, 7)), np.ones((npts, 3))))
+    res = types.SimpleNamespace(initial_cost=2.0, final_cost=1.0, iterations=10, accepted=9, pcg_iterations=50)
+    bench.dump_outputs(str(tmp_path), feats, graph, res)
+    want = {"keypoints": ((n, 7), np.float32), "descriptors": ((n, 32), np.float32), "match_index": ((n,), np.float32),
+            "match_distance": ((n,), np.float32), "match_distance2": ((n,), np.float32), "ba_poses_wc": ((nc, 7), np.float64),
+            "ba_points": ((npts, 3), np.float64), "ba_result": ((5,), np.float64)}
+    assert sorted(os.listdir(tmp_path)) == sorted(k + ".npy" for k in want)
+    for name, (shape, dtype) in want.items():
+        a = np.load(tmp_path / (name + ".npy"))
+        assert a.shape == shape and a.dtype == dtype, name
+    assert np.array_equal(np.load(tmp_path / "keypoints.npy")[:, 0], np.arange(n)) and (np.load(tmp_path / "keypoints.npy")[:, 5] == 2).all()
+    assert np.load(tmp_path / "ba_result.npy").tolist() == [2.0, 1.0, 10.0, 9.0, 50.0]
+
+
+def test_zero_steps_are_refused():
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--steps", "0"], capture_output=True, text=True, timeout=300, cwd=ROOT)
+    assert r.returncode != 0 and "--steps" in r.stderr

@@ -124,7 +124,7 @@ d.close(); dist.destroy_process_group()
 def test_world2_nccl_global_ba_matches_oracle(tmp_path):
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     script = tmp_path / "worker.py"
     script.write_text(GPU_WORKER)
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",

@@ -31,7 +31,7 @@ def test_against_numpy_popcount():
     assert np.array_equal(d2, np.sort(d, axis=1)[:, 1])
 
 
-@pytest.mark.skipif(not oracle.have_ref(), reason="oracle/_ref not built (needs /root/reference)")
+@pytest.mark.skipif(not oracle.have_ref(), reason="oracle/_ref not built (needs a GSLAM checkout)")
 def test_against_reference_hamming32_live():
     q = synth.random_descriptors(1000, 42); t = synth.random_descriptors(1000, 43)
     R = oracle.ref(); L = oracle.lib()

@@ -1,8 +1,10 @@
 """Pose-graph terms of the BundleGraph (SURVEY.md section 8f-3: GSLAM::SE3Edge / GPSEdge, Optimizer.h:127-148) in the BA oracle
 (oracle/ba_ref.c).  PARITY UNPINNED by reference tests (the reference has no optimiser); pinned here: the SE3 logarithm and product
-against the reference's own SE3 class (oracle/_ref), the edge conventions against the reference's comments (SE3_12 = SE3_1^-1 SE3_2:
+against the reference's own SE3 class (oracle/_ref, or its stored outputs), the edge conventions against the reference's comments (SE3_12 = SE3_1^-1 SE3_2:
 zero residual on consistent measurements), the gradient against central differences of the cost, and the optimum against an
 independent scipy least-squares on the stacked residuals."""
+import os
+
 import numpy as np
 import pytest
 
@@ -25,18 +27,32 @@ def retract_wc(pose_wc, d):
 
 
 def test_se3_log_and_product_equal_the_reference_class():
-    if not oracle.have_ref():
-        pytest.skip("oracle/_ref not built")
-    rng = np.random.default_rng(0)
-    R = O.ref()
-    for k in range(200):
-        scale = [1e-12, 1e-6, 0.3, 2.5][k % 4]
-        a = synth._small_se3(rng, 1, 1.0, scale)[0]; b = synth._small_se3(rng, 1, 2.0, 1.0)[0]
-        if k % 7 == 0:
-            a[:4] = -a[:4]                                     # the other quaternion of the same rotation
-        want = np.zeros(6); R.ref_se3_log(a.ctypes.data, want.ctypes.data)
+    """Against the reference's SE3 log and product: live where oracle/_ref is built (which must still give the stored values), else
+    as stored from it in tests/golden/reference_outputs.npz."""
+    G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_outputs.npz"))
+    A, B, LOG, MUL = [list(np.ascontiguousarray(x)) for x in (G["pg_a"], G["pg_b"], G["pg_log"], G["pg_mul"])]
+
+    def reference(R, a, b):
+        lg = np.zeros(6); R.ref_se3_log(a.ctypes.data, lg.ctypes.data)
+        m = np.zeros(7); R.ref_se3_mul(a.ctypes.data, b.ctypes.data, m.ctypes.data)
+        return lg, m
+    if oracle.have_ref():                     # the stored cases live, and 200 more random ones
+        R = O.ref()
+        for a, b, lg, m in zip(A, B, LOG, MUL):
+            live, lm = reference(R, a, b)
+            assert np.array_equal(live, lg) and np.array_equal(lm, m)
+        rng = np.random.default_rng(10)
+        for k in range(200):
+            scale = [1e-12, 1e-6, 0.3, 2.5][k % 4]
+            a = synth._small_se3(rng, 1, 1.0, scale)[0]; b = synth._small_se3(rng, 1, 2.0, 1.0)[0]
+            if k % 7 == 0:
+                a[:4] = -a[:4]                # the other quaternion of the same rotation
+            a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
+            lg, m = reference(R, a, b)
+            A.append(a); B.append(b); LOG.append(lg); MUL.append(m)
+    for a, b, want, wm in zip(A, B, LOG, MUL):
+        a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
         assert np.allclose(O.se3_log(a), want, rtol=0, atol=1e-14)
-        wm = np.zeros(7); R.ref_se3_mul(a.ctypes.data, b.ctypes.data, wm.ctypes.data)
         assert np.allclose(O.se3_mul(a, b), wm, rtol=0, atol=1e-14)
         assert np.allclose(synth.se3_mul(a, b), wm, rtol=0, atol=1e-13)     # the generator's numpy algebra too
 

@@ -15,7 +15,7 @@ ATAN = [W, H, 256.0, 252.0, 160.0, 120.0, 0.9]                                  
 
 def _need_ref():
     if not oracle.have_ref():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
+        pytest.skip("oracle/_ref not built (needs a GSLAM checkout)")
 
 
 def _frame(ch):
@@ -64,7 +64,7 @@ def test_remap_last_row_taps_count_as_zero():
 
 def test_remap_restatement_equals_the_committed_reference_vectors():
     """tests/golden/remap_opencv_96x72.npz was written by the reference itself (make_golden_remap.py); this runs on boxes
-    without /root/reference too."""
+    without the reference too."""
     import os
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", "remap_opencv_96x72.npz"))
     h, w = g["out1"].shape

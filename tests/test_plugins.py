@@ -12,11 +12,11 @@ import pytest
 import oracle
 from gslam_b200 import capi, synth
 
-LIB = os.path.join(os.path.dirname(capi.LIB_PATH))
+LIB = oracle.PLUGIN_DIR
 EXE = os.path.join(LIB, "gslam_b200_host_test")
 needs_plugins = pytest.mark.skipif(not all(os.path.exists(os.path.join(LIB, f)) for f in
                                            ("gslam_b200_host_test", "libgslam_optimizer.so", "libgslam_b200.so")),
-                                   reason="plugins not built (they need the reference headers: built in the build container)")
+                                   reason="oracle/_ref/plugins not built (they need the headers of a GSLAM checkout at build time)")
 
 
 def write_ba(path, pb, iters, ftol, edges=None):
@@ -231,7 +231,7 @@ def test_synth_dataset_frames_equal_python_generator(tmp_path):
 @pytest.mark.gpu
 def test_features_app_over_messenger_matches_direct_calls(tmp_path):
     """The Messenger-level pipeline of SURVEY.md 8f-2, wired like `gslam play b200_features -dataset x.synth`: dataset/frame ->
-    gslam.apps.b200_features (ORB extract on the B200, MapFrame::setKeyPoints, Hamming match against the previous frame) ->
+    gslam.apps.b200_features (ORB extract on the GPU, MapFrame::setKeyPoints, Hamming match against the previous frame) ->
     b200/curframe.  Every frame's keypoints / descriptors / matches equal direct C-ABI calls on the same frames."""
     from gslam_b200.api import Context
     cfg = tmp_path / "x.synth"

@@ -1,5 +1,4 @@
-"""GPU parity of gb_pnp_ransac and of Estimator::findPnP through the reference API against oracle/pnp_ref.c (first seen green on a
-B200 in round 2: tools/gpu_pnp_check.py, 30/30 cases, profiles/r02_pnp_check.log).
+"""GPU parity of gb_pnp_ransac and of Estimator::findPnP through the reference API against oracle/pnp_ref.c.
 
 Bar: same number of counted hypotheses, same winning hypothesis and root, identical inlier mask, pose within 1e-7 (the refinement is an LM solve on both sides: agreement at its convergence level; the minimal
 solver runs in fp64 on both sides with contraction disabled; only libm-vs-CUDA-math ulp differences in acos/cos/cbrt can move a
@@ -16,7 +15,7 @@ import oracle
 from gslam_b200 import capi
 
 pytestmark = pytest.mark.gpu
-LIB = os.path.dirname(capi.LIB_PATH)
+LIB = oracle.PLUGIN_DIR
 EXE = os.path.join(LIB, "gslam_b200_host_test")
 
 

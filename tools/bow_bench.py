@@ -28,6 +28,6 @@ for k, L in ((10, 4), (10, 5), (10, 6)):
         R.close()
     else:
         t0 = time.perf_counter(); O.bow_transform(v, f, 2); t_ref = time.perf_counter() - t0; kind = "oracle port"
-    print(f"k={k} L={L} ({v.n_nodes} nodes): parity {ok}; B200 {t_gpu * 1e6:.1f} us per 2000-descriptor transform (host in, host out, python call included); "
+    print(f"k={k} L={L} ({v.n_nodes} nodes): parity {ok}; GPU {t_gpu * 1e6:.1f} us per 2000-descriptor transform (host in, host out, python call included); "
           f"{kind} {t_ref * 1e6:.1f} us", flush=True)
     dv.close()
