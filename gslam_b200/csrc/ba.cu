@@ -7,10 +7,13 @@
 //                             ever materialised.
 //   K6b ba_linearize_cams   : one CTA per camera over its (camera-sorted) observation list, recomputing the residual,
 //                             fixed-tree block reduction -> U_i (6x6), g_c,i.  Deterministic (no atomics).
-//   K7a ba_point_inv / ba_schur_init / ba_schur_accum : damped V^-1, S = U - sum_j W V^-1 W', g~ = g_c - sum W V^-1 g_p.
-//   K7b pcg_init / pcg_matvec / pcg_update : block-Jacobi PCG on the reduced camera system, convergence decided on device.
-//   ba_backsub / ba_retract / ba_cost_points / ba_commit / ba_apply : back-substitution, candidate estimate, LM accept/reject.
-// All LM state lives in BaScalars on the device; kernels early-exit on its flags, so an iteration needs no host sync.
+//   K7a ba_prepare_schur / ba_schur_blocks (or _chunks + _reduce, or _accum + ba_mirror) : damped V^-1,
+//                             S = U - sum_j W V^-1 W', g~ = g_c - sum W V^-1 g_p.
+//   K7b ba_damp / pcg_init / pcg_matvec / pcg_update / ba_retract : block-Jacobi PCG on the reduced camera system, convergence
+//                             decided on device, candidate camera poses.
+//   ba_backsub_cost / ba_reduce_cost / ba_commit_apply : back-substitution + candidate cost, LM accept/reject + install.
+// All LM state lives in BaScalars on the device; kernels early-exit on its flags, so an iteration needs no host sync.  The LM rules
+// themselves (decision, damping, preconditioner, retraction, V^-1) are the helpers of ba_device.cuh, shared by every solver path.
 #include "ba_device.cuh"
 #include "common.cuh"
 #include "ba_internal.cuh"
@@ -161,21 +164,7 @@ __device__ __forceinline__ void ba_linearize_points_body(const BaDev& g, int blo
     g.gp[3 * (size_t)j] = acc[6]; g.gp[3 * (size_t)j + 1] = acc[7]; g.gp[3 * (size_t)j + 2] = acc[8];
     g.cost_pt[j] = acc[9];
     // damped inverse right away (ba_prepare_schur_kernel redoes it only when a rejected step changed lambda)
-    const double lambda = g.sc->lambda;
-    double Vi[9];
-    const bool active = pf && e1 > e0;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) Vi[k] = active ? V[k] : 0.0;
-    if (active) {
-#pragma unroll
-      for (int a = 0; a < 3; ++a) Vi[a * 4] += lambda * clampd(Vi[a * 4]);
-      if (!spd_inverse<3>(Vi)) {
-#pragma unroll
-        for (int k = 0; k < 9; ++k) Vi[k] = 0.0;
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < 9; ++k) g.Vinv[9 * (size_t)j + k] = Vi[k];
+    damped_vinv(V, pf && e1 > e0, g.sc->lambda, g.Vinv + 9 * (size_t)j);
   }
 }
 
@@ -641,9 +630,8 @@ __global__ void ba_damp_kernel(BaDev g, double* __restrict__ buf) {
   if (d >= g.n6) return;
   const size_t n6 = g.n6;
   const int i = d / 6, a = d % 6;
-  const double lambda = g.sc->lambda;
-  if ((g.dof[i] >> a) & 1) buf[(size_t)d * n6 + d] += lambda * clampd(buf[n6 * n6 + n6 + d]);
-  else buf[(size_t)d * n6 + d] = 1.0;
+  double* s = buf + (size_t)d * n6 + d;
+  *s = lm_damp(*s, buf[n6 * n6 + n6 + d], g.sc->lambda, (g.dof[i] >> a) & 1);
 }
 
 // ---- PCG ---------------------------------------------------------------------------------------------------------------
@@ -658,12 +646,7 @@ __global__ void __launch_bounds__(kRedThreads) pcg_init_kernel(BaDev g, const do
     for (int a = 0; a < 6; ++a)
 #pragma unroll
       for (int b = 0; b < 6; ++b) M[a * 6 + b] = S[(size_t)(6 * i + a) * n6 + 6 * i + b];
-    if (!spd_inverse<6>(M)) {
-#pragma unroll
-      for (int a = 0; a < 6; ++a)
-#pragma unroll
-        for (int b = 0; b < 6; ++b) M[a * 6 + b] = (a == b) ? 1.0 / S[(size_t)(6 * i + a) * n6 + 6 * i + a] : 0.0;
-    }
+    block_jacobi_inverse(M, S + (size_t)(6 * i) * n6 + 6 * i, n6);
 #pragma unroll
     for (int k = 0; k < 36; ++k) g.Minv[36 * (size_t)i + k] = M[k];
   }
@@ -772,98 +755,22 @@ __global__ void ba_retract_kernel(BaDev g) {
   if (g.sc->stop) return;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= g.nc) return;
-  double pose[7], d[6], out[7], R[9];
-  const int dm = g.dof[i];
-#pragma unroll
-  for (int k = 0; k < 7; ++k) pose[k] = g.pose[7 * i + k];
-#pragma unroll
-  for (int a = 0; a < 6; ++a) d[a] = ((dm >> a) & 1) ? g.x[6 * i + a] : 0.0;
-  se3_retract(pose, d, out);
-#pragma unroll
-  for (int k = 0; k < 7; ++k) g.pose_new[7 * i + k] = out[k];
-  quat_to_R(out, R);
-#pragma unroll
-  for (int k = 0; k < 9; ++k) g.Rt_new[12 * i + k] = R[k];
-#pragma unroll
-  for (int k = 0; k < 3; ++k) g.Rt_new[12 * i + 9 + k] = out[4 + k];
+  retract_camera(g, i, g.x + 6 * i);
 }
 
-// LM accept / reject from the (possibly all-reduced) costs
-__global__ void ba_commit_kernel(BaDev g, const double* __restrict__ buf, const double* __restrict__ d_cost) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  BaScalars* sc = g.sc;
-  if (sc->stop) return;
-  const size_t n6 = g.n6;
-  const double cost = buf[g.r_gt + 2 * n6], cnew = d_cost[0];
-  if (sc->iterations == 0) sc->initial_cost = cost;
-  sc->cost = cost;
-  sc->cost_new = cnew;
-  sc->iterations++;
-  const bool ok = (cnew < cost) && isfinite(cnew);
-  sc->accept_flag = ok ? 1 : 0;
-  sc->need_linearize = ok ? 1 : 0;
-  if (ok) {
-    const double rel = (cost - cnew) / cost;
-    sc->cost = cnew;
-    double l = sc->lambda / 3.0;
-    sc->lambda = l < 1e-15 ? 1e-15 : l;
-    sc->nu = 2.0;
-    sc->accepted++;
-    if (rel < sc->ftol) { sc->stop = 1; sc->status = 1; }
-  } else {
-    sc->lambda *= sc->nu;
-    sc->nu *= 2.0;
-    if (sc->lambda > 1e16) { sc->stop = 1; sc->status = 2; }
-  }
-}
-
-// LM accept / reject AND the installation of an accepted candidate in one launch (compact path).  Every thread derives the
-// decision from the two (possibly all-reduced) costs alone; only thread 0 of CTA 0 touches the LM scalars, so nobody reads what it
-// writes.  Re-running it after a stop is harmless: the candidate arrays are frozen once `stop` is set.
+// LM accept / reject AND the installation of an accepted candidate in one launch.  Every thread derives the decision from the two
+// (possibly all-reduced) costs alone; only thread 0 of CTA 0 touches the LM scalars, so nobody reads what it writes.  Re-running it
+// after a stop is harmless: the candidate arrays are frozen once `stop` is set.
 __global__ void ba_commit_apply_kernel(BaDev g, const double* __restrict__ buf, const double* __restrict__ d_cost) {
   const size_t n6 = g.n6;
   const double cost = buf[g.r_gt + 2 * n6], cnew = d_cost[0];
-  const bool ok = (cnew < cost) && isfinite(cnew);
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    BaScalars* sc = g.sc;
-    if (!sc->stop) {
-      if (sc->iterations == 0) sc->initial_cost = cost;
-      sc->cost = cost;
-      sc->cost_new = cnew;
-      sc->iterations++;
-      sc->need_linearize = ok ? 1 : 0;
-      if (ok) {
-        const double rel = (cost - cnew) / cost;
-        sc->cost = cnew;
-        const double l = sc->lambda / 3.0;
-        sc->lambda = l < 1e-15 ? 1e-15 : l;
-        sc->nu = 2.0;
-        sc->accepted++;
-        if (rel < sc->ftol) { sc->stop = 1; sc->status = 1; }
-      } else {
-        sc->lambda *= sc->nu;
-        sc->nu *= 2.0;
-        if (sc->lambda > 1e16) { sc->stop = 1; sc->status = 2; }
-      }
-    }
-  }
+  const bool ok = (blockIdx.x == 0 && threadIdx.x == 0 && !g.sc->stop) ? lm_decide(g.sc, cost, cnew) : lm_accepts(cost, cnew);
   if (!ok) return;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < g.nc * 7) g.pose[t] = g.pose_new[t];
   if (t < g.nc * 12) g.Rt[t] = g.Rt_new[t];
   if (t < g.np * 3) g.pts[t] = g.pts_new[t];
 }
-
-// on accept: estimate <- candidate.  (runs even when ba_commit just set stop: the accepted step must land)
-__global__ void ba_apply_kernel(BaDev g) {
-  if (!g.sc->accept_flag) return;
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t < g.nc * 7) g.pose[t] = g.pose_new[t];
-  if (t < g.nc * 12) g.Rt[t] = g.Rt_new[t];
-  if (t < g.np * 3) g.pts[t] = g.pts_new[t];
-}
-
-__global__ void ba_clear_accept_kernel(BaScalars* sc) { sc->accept_flag = 0; }
 
 __global__ void ba_finalize_kernel(int nc, const double* __restrict__ pose_cw, double* __restrict__ pose_wc) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -896,39 +803,20 @@ __global__ void __launch_bounds__(256) ba_prepare_schur_kernel(BaDev g, double* 
   }
   const double lambda = g.sc->lambda;
   const bool fresh = g.sc->need_linearize != 0 && g.vinv_in_sweep != 0;  // the sweep of this iteration already produced Vinv with this lambda
-  for (size_t j = t0; !fresh && j < (size_t)g.np; j += stride) {
-    double Vi[9];
-    const bool active = g.pfree[j] != 0 && g.pt_off[j + 1] > g.pt_off[j];
-#pragma unroll
-    for (int k = 0; k < 9; ++k) Vi[k] = active ? g.V[9 * j + k] : 0.0;
-    if (active) {
-#pragma unroll
-      for (int a = 0; a < 3; ++a) Vi[a * 4] += lambda * clampd(Vi[a * 4]);
-      if (!spd_inverse<3>(Vi)) {
-#pragma unroll
-        for (int k = 0; k < 9; ++k) Vi[k] = 0.0;
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < 9; ++k) g.Vinv[9 * j + k] = Vi[k];
-  }
+  for (size_t j = t0; !fresh && j < (size_t)g.np; j += stride)
+    damped_vinv(g.V + 9 * j, g.pfree[j] != 0 && g.pt_off[j + 1] > g.pt_off[j], lambda, g.Vinv + 9 * j);
   // deterministic cost reduction over the whole grid (every block adds a slice, the last one folds the partials in block order)
   __shared__ int s_flag;
   grid_sum_to<256>(g.cost_pt, g.np + g.npe, 0.5, g.red_part, g.red_ticket, buf + g.r_gt + 2 * n6, s_part, &s_flag);
 }
 
-// back-substitution of landmark j followed by its robustified cost at the candidate estimate; 8 lanes per landmark
-__global__ void __launch_bounds__(128) ba_backsub_cost_kernel(BaDev g) {
-  if (g.sc->stop) return;
-  const int gt = blockIdx.x * blockDim.x + threadIdx.x;
-  const int jraw = gt / kLpp, sub = gt % kLpp;
-  const bool valid = jraw < g.np;
-  const int j = valid ? jraw : 0;
-  const double delta = g.sc->delta;
-  const int e0 = g.pt_off[j], e1 = valid ? g.pt_off[j + 1] : e0;
+// Back-substitution of landmark j followed by its robustified cost at the candidate estimate -> pts_new[j], cost_pt_new[j].  kLpp
+// lanes per landmark: lane `sub` takes observations e0 + sub, e0 + sub + kLpp, ... of the landmark's segment [e0, e1); i_first is the
+// camera of its first one (o_cam[e0 + sub]), which the caller may request early.
+__device__ __forceinline__ void ba_backsub_cost(const BaDev& g, int j, bool valid, int sub, int e0, int e1, int i_first, double delta) {
   double b[3] = {0.0, 0.0, 0.0};
   for (int e = e0 + sub; e < e1; e += kLpp) {
-    const int i = g.o_cam[e];
+    const int i = (e == e0 + sub) ? i_first : g.o_cam[e];
     const double* W = g.W + 18 * (size_t)e;
 #pragma unroll
     for (int c = 0; c < 3; ++c)
@@ -947,7 +835,8 @@ __global__ void __launch_bounds__(128) ba_backsub_cost_kernel(BaDev g) {
   for (int a = 0; a < 3; ++a) p[a] = g.pts[3 * (size_t)j + a] + Vi[a * 3] * b[0] + Vi[a * 3 + 1] * b[1] + Vi[a * 3 + 2] * b[2];
   double cost = 0.0;
   for (int e = e0 + sub; e < e1; e += kLpp) {
-    const ObsLin o = eval_obs(g.Rt_new + 12 * g.o_cam[e], p, g.o_uv[2 * e], g.o_uv[2 * e + 1], g.has_info ? g.o_info + 3 * e : nullptr, delta);
+    const int i = (e == e0 + sub) ? i_first : g.o_cam[e];
+    const ObsLin o = eval_obs(g.Rt_new + 12 * i, p, g.o_uv[2 * e], g.o_uv[2 * e + 1], g.has_info ? g.o_info + 3 * e : nullptr, delta);
     cost += o.rho;
   }
 #pragma unroll
@@ -959,10 +848,21 @@ __global__ void __launch_bounds__(128) ba_backsub_cost_kernel(BaDev g) {
   }
 }
 
+__global__ void __launch_bounds__(128) ba_backsub_cost_kernel(BaDev g) {
+  if (g.sc->stop) return;
+  const int gt = blockIdx.x * blockDim.x + threadIdx.x;
+  const int jraw = gt / kLpp, sub = gt % kLpp;
+  const bool valid = jraw < g.np;
+  const int j = valid ? jraw : 0;
+  const double delta = g.sc->delta;
+  const int e0 = g.pt_off[j], e1 = valid ? g.pt_off[j + 1] : e0;
+  ba_backsub_cost(g, j, valid, sub, e0, e1, (e0 + sub < e1) ? g.o_cam[e0 + sub] : 0, delta);
+}
+
 // Local-BA tail in ONE launch: back-substitution + candidate cost (8 lanes per landmark), then the LAST CTA to finish
 // (atomic ticket) reduces both costs in a fixed order, takes the LM accept/reject decision, and either installs the candidate
 // (accept) or refreshes the damped V^-1 with the new lambda (reject: the next iteration skips the sweep).  Replaces
-// ba_prepare_schur + ba_backsub_cost + ba_commit_fused on the block-CSR path.
+// ba_prepare_schur + ba_backsub_cost + ba_reduce_cost + ba_commit_apply of the stepwise path.
 constexpr int kTailThreads = 256;
 // CTA-wide copy of n doubles (16-byte accesses; both pointers are slab-aligned)
 __device__ __forceinline__ void cta_copy_f64(double* __restrict__ dst, const double* __restrict__ src, int n, int nthreads) {
@@ -985,42 +885,8 @@ __global__ void __launch_bounds__(kTailThreads) ba_backsub_commit_kernel(BaDev g
   const int i_first = (e0 + sub < e1) ? g.o_cam[e0 + sub] : 0;
   gb_pdl_wait();
   if (sc->stop) return;
-  {  // ---- part 1: identical to ba_backsub_cost_kernel
-    const double delta = sc->delta;
-    double b[3] = {0.0, 0.0, 0.0};
-    for (int e = e0 + sub; e < e1; e += kLpp) {
-      const int i = (e == e0 + sub) ? i_first : g.o_cam[e];
-      const double* W = g.W + 18 * (size_t)e;
-#pragma unroll
-      for (int c = 0; c < 3; ++c)
-#pragma unroll
-        for (int a = 0; a < 6; ++a) b[c] -= W[a * 3 + c] * g.x[6 * i + a];
-    }
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-#pragma unroll
-      for (int o = kLpp / 2; o > 0; o >>= 1) b[c] += __shfl_xor_sync(0xffffffffu, b[c], o, kLpp);
-      b[c] += g.gp[3 * (size_t)j + c];
-    }
-    const double* Vi = g.Vinv + 9 * (size_t)j;
-    double p[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) p[a] = g.pts[3 * (size_t)j + a] + Vi[a * 3] * b[0] + Vi[a * 3 + 1] * b[1] + Vi[a * 3 + 2] * b[2];
-    double cost = 0.0;
-    for (int e = e0 + sub; e < e1; e += kLpp) {
-      const int i = (e == e0 + sub) ? i_first : g.o_cam[e];
-      const ObsLin o = eval_obs(g.Rt_new + 12 * i, p, g.o_uv[2 * e], g.o_uv[2 * e + 1], g.has_info ? g.o_info + 3 * e : nullptr, delta);
-      cost += o.rho;
-    }
-#pragma unroll
-    for (int o = kLpp / 2; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o, kLpp);
-    if (valid && sub == 0) {
-#pragma unroll
-      for (int a = 0; a < 3; ++a) g.pts_new[3 * (size_t)j + a] = p[a];
-      g.cost_pt_new[j] = cost;
-    }
-  }
-  // ---- part 2: last CTA done
+  ba_backsub_cost(g, j, valid, sub, e0, e1, i_first, sc->delta);
+  // ---- the last CTA done: both costs, the LM decision, install or V^-1 refresh
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) s_flag = (atomicAdd(&sc->ticket, 1u) == gridDim.x - 1) ? 1 : 0;
@@ -1036,48 +902,15 @@ __global__ void __launch_bounds__(kTailThreads) ba_backsub_commit_kernel(BaDev g
   const double cnew = 0.5 * block_sum<kTailThreads>(v1, s_part);
   if (threadIdx.x == 0) {
     sc->ticket = 0;
-    if (sc->iterations == 0) sc->initial_cost = cost;
-    sc->cost = cost;
-    sc->cost_new = cnew;
-    sc->iterations++;
-    const bool ok = (cnew < cost) && isfinite(cnew);
-    sc->need_linearize = ok ? 1 : 0;
-    if (ok) {
-      const double rel = (cost - cnew) / cost;
-      sc->cost = cnew;
-      const double l = sc->lambda / 3.0;
-      sc->lambda = l < 1e-15 ? 1e-15 : l;
-      sc->nu = 2.0;
-      sc->accepted++;
-      if (rel < sc->ftol) { sc->stop = 1; sc->status = 1; }
-    } else {
-      sc->lambda *= sc->nu;
-      sc->nu *= 2.0;
-      if (sc->lambda > 1e16) { sc->stop = 1; sc->status = 2; }
-    }
-    s_flag = ok ? 2 : 1;
+    s_flag = lm_decide(sc, cost, cnew) ? 2 : 1;
   }
   __syncthreads();
   if (s_flag == 2) {  // accept: the next sweep reads the candidate arrays and installs them on the fly (no serial copy here)
     if (threadIdx.x == 0) sc->pending = 1;
   } else {  // reject: same linearisation, new lambda -> refresh the damped landmark inverses
     const double lambda = sc->lambda;
-    for (int j = threadIdx.x; j < g.np; j += kTailThreads) {
-      double Vi[9];
-      const bool active = g.pfree[j] != 0 && g.pt_off[j + 1] > g.pt_off[j];
-#pragma unroll
-      for (int k = 0; k < 9; ++k) Vi[k] = active ? g.V[9 * (size_t)j + k] : 0.0;
-      if (active) {
-#pragma unroll
-        for (int a = 0; a < 3; ++a) Vi[a * 4] += lambda * clampd(Vi[a * 4]);
-        if (!spd_inverse<3>(Vi)) {
-#pragma unroll
-          for (int k = 0; k < 9; ++k) Vi[k] = 0.0;
-        }
-      }
-#pragma unroll
-      for (int k = 0; k < 9; ++k) g.Vinv[9 * (size_t)j + k] = Vi[k];
-    }
+    for (int j = threadIdx.x; j < g.np; j += kTailThreads)
+      damped_vinv(g.V + 9 * (size_t)j, g.pfree[j] != 0 && g.pt_off[j + 1] > g.pt_off[j], lambda, g.Vinv + 9 * (size_t)j);
   }
 }
 
@@ -1093,46 +926,6 @@ __global__ void __launch_bounds__(1024) ba_install_pending_kernel(BaDev g) {
   cta_copy_f64(g.Rt, g.Rt_new, g.nc * 12, 1024);
   cta_copy_f64(g.pose, g.pose_new, g.nc * 7, 1024);
   if (threadIdx.x == 0) g.sc->pending = 0;
-}
-
-// single CTA: reduce the candidate cost, LM accept/reject, apply.  (small problems; the stepwise path keeps them apart)
-__global__ void __launch_bounds__(kRedThreads) ba_commit_fused_kernel(BaDev g, const double* __restrict__ buf) {
-  BaScalars* sc = g.sc;
-  if (sc->stop) return;
-  __shared__ double s_part[kRedThreads / 32 + 1];
-  __shared__ int s_ok;
-  double v = 0.0;
-  for (int k = threadIdx.x; k < g.np; k += kRedThreads) v += g.cost_pt_new[k];
-  const double cnew = 0.5 * block_sum<kRedThreads>(v, s_part);
-  if (threadIdx.x == 0) {
-    const size_t n6 = g.n6;
-    const double cost = buf[n6 * n6 + 2 * n6];
-    if (sc->iterations == 0) sc->initial_cost = cost;
-    sc->cost = cost;
-    sc->cost_new = cnew;
-    sc->iterations++;
-    const bool ok = (cnew < cost) && isfinite(cnew);
-    sc->need_linearize = ok ? 1 : 0;
-    if (ok) {
-      const double rel = (cost - cnew) / cost;
-      sc->cost = cnew;
-      const double l = sc->lambda / 3.0;
-      sc->lambda = l < 1e-15 ? 1e-15 : l;
-      sc->nu = 2.0;
-      sc->accepted++;
-      if (rel < sc->ftol) { sc->stop = 1; sc->status = 1; }
-    } else {
-      sc->lambda *= sc->nu;
-      sc->nu *= 2.0;
-      if (sc->lambda > 1e16) { sc->stop = 1; sc->status = 2; }
-    }
-    s_ok = ok ? 1 : 0;
-  }
-  __syncthreads();
-  if (!s_ok) return;
-  for (int t = threadIdx.x; t < g.nc * 7; t += kRedThreads) g.pose[t] = g.pose_new[t];
-  for (int t = threadIdx.x; t < g.nc * 12; t += kRedThreads) g.Rt[t] = g.Rt_new[t];
-  for (int t = threadIdx.x; t < g.np * 3; t += kRedThreads) g.pts[t] = g.pts_new[t];
 }
 
 // ---- K7b (local BA, sparse covisibility): block-Jacobi PCG in ONE CTA -------------------------------------------------------
@@ -1213,7 +1006,7 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
     int dblk = rowptr[i];
     while (col[dblk] != i) ++dblk;  // the diagonal block is always present
     const int w = dblk * 36 + a * 7;
-    const double v = ((g.dof[i] >> a) & 1) ? B[w] + lambda * clampd(buf[nS + n6 + d]) : 1.0;
+    const double v = lm_damp(B[w], buf[nS + n6 + d], lambda, (g.dof[i] >> a) & 1);
     B[w] = v;
     g.Sb[w] = v;
   }
@@ -1225,12 +1018,7 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
     double M[36];
 #pragma unroll
     for (int k = 0; k < 36; ++k) M[k] = B[(size_t)dblk * 36 + k];
-    if (!spd_inverse<6>(M)) {
-#pragma unroll
-      for (int a = 0; a < 6; ++a)
-#pragma unroll
-        for (int b = 0; b < 6; ++b) M[a * 6 + b] = (a == b) ? 1.0 / B[(size_t)dblk * 36 + a * 7] : 0.0;
-    }
+    block_jacobi_inverse(M, B + (size_t)dblk * 36, 6);
 #pragma unroll
     for (int k = 0; k < 36; ++k) Minv[36 * i + k] = M[k];
   }
@@ -1387,22 +1175,7 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
   if (tid == 0) g.sc->pcg_iters += iters;
   __syncthreads();
   for (int k = tid; k < n6; k += THREADS) g.x[k] = vx[k];
-  for (int i = tid; i < nc; i += THREADS) {
-    double pose[7], dd[6], out[7], R[9];
-    const int dm = g.dof[i];
-#pragma unroll
-    for (int k = 0; k < 7; ++k) pose[k] = g.pose[7 * i + k];
-#pragma unroll
-    for (int a = 0; a < 6; ++a) dd[a] = ((dm >> a) & 1) ? vx[6 * i + a] : 0.0;
-    se3_retract(pose, dd, out);
-#pragma unroll
-    for (int k = 0; k < 7; ++k) g.pose_new[7 * i + k] = out[k];
-    quat_to_R(out, R);
-#pragma unroll
-    for (int k = 0; k < 9; ++k) g.Rt_new[12 * i + k] = R[k];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) g.Rt_new[12 * i + 9 + k] = out[4 + k];
-  }
+  for (int i = tid; i < nc; i += THREADS) retract_camera(g, i, vx + 6 * i);
 }
 constexpr int kSpSmallCams = 48;     // active cameras of the 12-warp variant (168 registers, 7 register columns per lane)
 constexpr int kSpMaxCams = 80;       // active cameras of the 20-warp variant (96 registers, 5 register columns per lane)
@@ -1441,7 +1214,7 @@ __global__ void __launch_bounds__(kPcgThreads, 1) ba_pcg_cluster_kernel(BaDev g,
     const int row = idx / n6, col = idx - row * n6, d = r0 + row;
     double v = buf[(size_t)d * n6 + col];
     if (col == d) {
-      v = ((g.dof[d / 6] >> (d % 6)) & 1) ? v + lambda * clampd(buf[nS + n6 + d]) : 1.0;
+      v = lm_damp(v, buf[nS + n6 + d], lambda, (g.dof[d / 6] >> (d % 6)) & 1);
       buf[(size_t)d * n6 + col] = v;
     }
     S[idx] = v;
@@ -1454,12 +1227,7 @@ __global__ void __launch_bounds__(kPcgThreads, 1) ba_pcg_cluster_kernel(BaDev g,
     for (int a = 0; a < 6; ++a)
 #pragma unroll
       for (int b = 0; b < 6; ++b) M[a * 6 + b] = S[(size_t)(6 * tid + a) * n6 + r0 + 6 * tid + b];
-    if (!spd_inverse<6>(M)) {
-#pragma unroll
-      for (int a = 0; a < 6; ++a)
-#pragma unroll
-        for (int b = 0; b < 6; ++b) M[a * 6 + b] = (a == b) ? 1.0 / S[(size_t)(6 * tid + a) * n6 + r0 + 6 * tid + a] : 0.0;
-    }
+    block_jacobi_inverse(M, S + (size_t)(6 * tid) * n6 + r0 + 6 * tid, n6);
 #pragma unroll
     for (int k = 0; k < 36; ++k) g.Minv[36 * (size_t)(c0 + tid) + k] = M[k];
   }
@@ -1589,22 +1357,7 @@ __global__ void __launch_bounds__(kPcgThreads, 1) ba_pcg_cluster_kernel(BaDev g,
   // D. CTA 0 publishes the solution, the iteration count and the candidate camera poses
   for (int d = tid; d < n6; d += kPcgThreads) g.x[d] = vx[d];
   if (tid == 0) g.sc->pcg_iters += iters;
-  for (int i = tid; i < nc; i += kPcgThreads) {
-    double pose[7], dd[6], out[7], R[9];
-    const int dm = g.dof[i];
-#pragma unroll
-    for (int k = 0; k < 7; ++k) pose[k] = g.pose[7 * i + k];
-#pragma unroll
-    for (int a = 0; a < 6; ++a) dd[a] = ((dm >> a) & 1) ? vx[6 * i + a] : 0.0;
-    se3_retract(pose, dd, out);
-#pragma unroll
-    for (int k = 0; k < 7; ++k) g.pose_new[7 * i + k] = out[k];
-    quat_to_R(out, R);
-#pragma unroll
-    for (int k = 0; k < 9; ++k) g.Rt_new[12 * i + k] = R[k];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) g.Rt_new[12 * i + 9 + k] = out[4 + k];
-  }
+  for (int i = tid; i < nc; i += kPcgThreads) retract_camera(g, i, vx + 6 * i);
 }
 
 }  // namespace
@@ -1986,7 +1739,7 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   const int np = hi - lo, no = e_hi - e_lo;
   d.nc = nc; d.np = np; d.no = no; d.n6 = 6 * nc; d.has_info = pb->obs_info ? 1 : 0;
   d.vinv_in_sweep = 1;
-  d.r_gt = (size_t)d.n6 * d.n6;  // dense layout unless a launch says otherwise (ba_reduce_local_compact / ba_commit_compact)
+  d.r_gt = (size_t)d.n6 * d.n6;  // dense layout unless a launch says otherwise (ba_compact_iteration)
   g->buf_doubles = ba_buf_doubles(nc);
   // covisibility block structure of S over the WHOLE graph (every rank of a sharded solve must agree on the layout): block
   // (i,i') is structurally non-zero iff some landmark is seen by both cameras
@@ -2289,7 +2042,7 @@ static int ba_pcg_cluster(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
 // bandwidth-tuned persistent kernel (ba_sweep.cu), small ones the latency-tuned one above.  which: 3 whole, 1 cameras, 2 landmarks.
 constexpr int kSweepLargeObs = 65536;
 static bool ba_sweep_is_large(const gb_ba_graph* g) {
-  return g->sweep_mode == 2 || (g->sweep_mode == 0 && g->d.no >= kSweepLargeObs && !getenv("GB_BA_SWEEP_OLD"));
+  return g->sweep_mode == 2 || (g->sweep_mode == 0 && g->d.no >= kSweepLargeObs);
 }
 static int ba_launch_sweep(gb_ctx* ctx, gb_ba_graph* g, const BaDev& d, cudaStream_t s, int which) {
   if (ba_sweep_is_large(g)) return ba_sweep_launch(ctx, g, d, s, which);
@@ -2353,109 +2106,82 @@ int gb_ba_graph_reduce_local(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
 
 }  // extern "C"
 
-// ---- the LM iteration on the COMPACT reduced layout rbuf = [Sb (nnzb x 36) | g~ | diag U | cost | pad] ------------------------------
-// (large graphs on one GPU and every rank of the landmark-sharded solve: the shard's contribution is what the collective sums)
-int ba_reduce_local_compact(gb_ctx* ctx, gb_ba_graph* g, double* rbuf) {
-  if (!ctx || !g || !g->begun || !rbuf || g->d.s_nnzb <= 0) return GB_ERR_INVALID;
-  CtxLock lk(ctx);
+static int ba_red_blocks(const gb_ctx* ctx, int n) { return std::max(1, std::min(std::min(ctx->sm_count, kRedPartials), (n + 8 * kRedThreads - 1) / (8 * kRedThreads))); }
+
+// ---- one LM iteration on the COMPACT reduced layout rbuf = [Sb (nnzb x 36) | g~ | diag U | cost | pad] ------------------------------
+// (large graphs on one GPU and every rank of the landmark-sharded solve: with a communicator, what the collective sums is the shard's
+// contribution to the reduced system and to the candidate cost)
+int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
   BaDev d = g->d;
-  d.Sb = rbuf;
+  d.Sb = g->rbuf;
   d.r_gt = (size_t)d.s_nnzb * 36;
-  cudaStream_t s = ctx->stream;
   d.vinv_in_sweep = ba_sweep_is_large(g) ? 0 : 1;
+  cudaStream_t s = ctx->stream;
   GB_CHECK(ba_launch_sweep(ctx, g, d, s, 3));
   {
     const int nblk = (int)std::min<size_t>(std::max<size_t>(((size_t)d.np + 255) / 256, 1), (size_t)ctx->sm_count * 8);
-    ba_prepare_schur_kernel<<<nblk, 256, 0, s>>>(d, rbuf, 0); GB_LAUNCH_CHECK(ctx);
+    ba_prepare_schur_kernel<<<nblk, 256, 0, s>>>(d, g->rbuf, 0); GB_LAUNCH_CHECK(ctx);
   }
   if (d.sp_nchunks > 0) {
     ba_schur_chunks_kernel<<<d.sp_nchunks, kChunkThreads, 0, s>>>(d); GB_LAUNCH_CHECK(ctx);
-    ba_schur_reduce_kernel<<<d.s_nupper, 64, 0, s>>>(d, rbuf); GB_LAUNCH_CHECK(ctx);
+    ba_schur_reduce_kernel<<<d.s_nupper, 64, 0, s>>>(d, g->rbuf); GB_LAUNCH_CHECK(ctx);
   } else {
-    ba_schur_blocks_kernel<<<d.s_nupper, 128, 0, s>>>(d, rbuf); GB_LAUNCH_CHECK(ctx);
+    ba_schur_blocks_kernel<<<d.s_nupper, 128, 0, s>>>(d, g->rbuf); GB_LAUNCH_CHECK(ctx);
   }
-  return GB_OK;
-}
-
-static int ba_red_blocks(const gb_ctx* ctx, int n) { return std::max(1, std::min(std::min(ctx->sm_count, kRedPartials), (n + 8 * kRedThreads - 1) / (8 * kRedThreads))); }
-
-int ba_backsub_cost_compact(gb_ctx* ctx, gb_ba_graph* g, double* d_cost) {
-  if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
-  CtxLock lk(ctx);
-  BaDev& d = g->d;
-  if (!d_cost) d_cost = g->d_cost;
-  if (d.np > 0) { ba_backsub_cost_kernel<<<gb_div_up(d.np * kLpp, 128), 128, 0, ctx->stream>>>(d); GB_LAUNCH_CHECK(ctx); }
-  ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np), kRedThreads, 0, ctx->stream>>>(d, d.cost_pt_new, d.np, d_cost); GB_LAUNCH_CHECK(ctx);
-  return GB_OK;
-}
-
-int ba_commit_compact(gb_ctx* ctx, gb_ba_graph* g, const double* rbuf, const double* d_cost) {
-  if (!ctx || !g || !g->begun || !rbuf) return GB_ERR_INVALID;
-  CtxLock lk(ctx);
-  BaDev d = g->d;
-  d.r_gt = (size_t)d.s_nnzb * 36;
-  if (!d_cost) d_cost = g->d_cost;
-  cudaStream_t s = ctx->stream;
+  if (comm) GB_CHECK(gb_comm_allreduce_sum_f64(comm, g->rbuf, g->rbuf_doubles));
+  GB_CHECK(ba_pcg_bcsr_launch(ctx, g, g->rbuf));
+  if (d.np > 0) { ba_backsub_cost_kernel<<<gb_div_up(d.np * kLpp, 128), 128, 0, s>>>(d); GB_LAUNCH_CHECK(ctx); }
+  ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np), kRedThreads, 0, s>>>(d, d.cost_pt_new, d.np, g->d_cost); GB_LAUNCH_CHECK(ctx);
+  if (comm) GB_CHECK(gb_comm_allreduce_sum_f64(comm, g->d_cost, 1));
   const int n = std::max(std::max(d.nc * 12, d.np * 3), 1);
-  ba_commit_apply_kernel<<<gb_div_up(n, 256), 256, 0, s>>>(d, rbuf, d_cost); GB_LAUNCH_CHECK(ctx);
+  ba_commit_apply_kernel<<<gb_div_up(n, 256), 256, 0, s>>>(d, g->rbuf, g->d_cost); GB_LAUNCH_CHECK(ctx);
   return GB_OK;
 }
-
-int ba_read_result(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* res) { return gb_ba_graph_finish(ctx, g, res); }
 
 extern "C" {
 
-static int ba_pcg_dispatch(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
-  BaDev& d = g->d;
-  cudaStream_t s = ctx->stream;
-  if (d.nc <= 0) return GB_OK;
-  if (g->opt.linear_solver == 1) return ba_chol_launch(ctx, g, buf, false);
-  if (g->pcg_sparse && buf == g->buf) {
-    if (g->pcg_nact <= kSpSmallCams) {
-      BA_SPARSE_SMALL<<<1, kSpSmallThreads, g->pcg_sparse_smem, s>>>(d, buf, (int)g->opt.pcg_max_iters);
-    } else {
-      BA_SPARSE_LARGE<<<1, kSpLargeThreads, g->pcg_sparse_smem, s>>>(d, buf, (int)g->opt.pcg_max_iters);
-    }
-    GB_LAUNCH_CHECK(ctx);
-  } else if (g->pcg_cluster > 0) {
-    GB_CHECK(ba_pcg_cluster(ctx, g, buf));
-  } else {
-    GB_CHECK(ba_pcg_generic(ctx, g, buf));
-  }
+// single-CTA block-sparse PCG, in the variant that fits the graph's active cameras (pdl: programmatic dependent launch)
+static int ba_pcg_sparse_launch(gb_ctx* ctx, gb_ba_graph* g, double* buf, bool pdl) {
+  const bool small = g->pcg_nact <= kSpSmallCams;
+  void (*kernel)(BaDev, double*, int) = small ? BA_SPARSE_SMALL : BA_SPARSE_LARGE;
+  const dim3 block(small ? kSpSmallThreads : kSpLargeThreads);
+  const int maxit = (int)g->opt.pcg_max_iters;
+  if (pdl) GB_CUDA(ctx, gb_launch_pdl(kernel, dim3(1), block, g->pcg_sparse_smem, ctx->stream, g->d, buf, maxit));
+  else kernel<<<1, block, g->pcg_sparse_smem, ctx->stream>>>(g->d, buf, maxit);
+  GB_LAUNCH_CHECK(ctx);
   return GB_OK;
 }
 
-static int ba_step_core(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
-  BaDev& d = g->d;
-  cudaStream_t s = ctx->stream;
-  GB_CHECK(ba_pcg_dispatch(ctx, g, buf));
-  if (d.np > 0) { ba_backsub_cost_kernel<<<gb_div_up(d.np * kLpp, 128), 128, 0, s>>>(d); GB_LAUNCH_CHECK(ctx); }
-  return GB_OK;
+static int ba_pcg_dispatch(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
+  if (g->d.nc <= 0) return GB_OK;
+  if (g->opt.linear_solver == 1) return ba_chol_launch(ctx, g, buf, false);
+  if (g->pcg_sparse && buf == g->buf) return ba_pcg_sparse_launch(ctx, g, buf, false);
+  if (g->pcg_cluster > 0) return ba_pcg_cluster(ctx, g, buf);
+  return ba_pcg_generic(ctx, g, buf);
 }
 
 int gb_ba_graph_step(gb_ctx* ctx, gb_ba_graph* g, const double* buf_in, double* d_cost) {
   if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   BaDev& d = g->d;
+  cudaStream_t s = ctx->stream;
   double* buf = buf_in ? (double*)buf_in : g->buf;
   if (!d_cost) d_cost = g->d_cost;
-  GB_CHECK(ba_step_core(ctx, g, buf));
-  GB_CHECK(ba_pose_cost(ctx, g, ctx->stream));
-  ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np + d.npe), kRedThreads, 0, ctx->stream>>>(d, d.cost_pt_new, d.np + d.npe, d_cost); GB_LAUNCH_CHECK(ctx);
+  GB_CHECK(ba_pcg_dispatch(ctx, g, buf));
+  if (d.np > 0) { ba_backsub_cost_kernel<<<gb_div_up(d.np * kLpp, 128), 128, 0, s>>>(d); GB_LAUNCH_CHECK(ctx); }
+  GB_CHECK(ba_pose_cost(ctx, g, s));
+  ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np + d.npe), kRedThreads, 0, s>>>(d, d.cost_pt_new, d.np + d.npe, d_cost); GB_LAUNCH_CHECK(ctx);
   return GB_OK;
 }
 
 int gb_ba_graph_commit(gb_ctx* ctx, gb_ba_graph* g, const double* buf_in, const double* d_cost) {
   if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  BaDev& d = g->d;
+  BaDev& d = g->d;  // (dense layout: the cost sits at r_gt = n6 * n6)
   const double* buf = buf_in ? buf_in : g->buf;
   if (!d_cost) d_cost = g->d_cost;
-  cudaStream_t s = ctx->stream;
-  ba_commit_kernel<<<1, 32, 0, s>>>(d, buf, d_cost); GB_LAUNCH_CHECK(ctx);
   const int n = std::max(std::max(d.nc * 12, d.np * 3), 1);
-  ba_apply_kernel<<<gb_div_up(n, 256), 256, 0, s>>>(d); GB_LAUNCH_CHECK(ctx);
-  ba_clear_accept_kernel<<<1, 1, 0, s>>>(d.sc); GB_LAUNCH_CHECK(ctx);
+  ba_commit_apply_kernel<<<gb_div_up(n, 256), 256, 0, ctx->stream>>>(d, buf, d_cost); GB_LAUNCH_CHECK(ctx);
   return GB_OK;
 }
 
@@ -2465,11 +2191,8 @@ static int ba_read_scalars(gb_ctx* ctx, gb_ba_graph* g, BaScalars* out) {
   return GB_OK;
 }
 
-int gb_ba_graph_finish(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* res) {
-  if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
-  CtxLock lk(ctx);
-  BaScalars h;
-  GB_CHECK(ba_read_scalars(ctx, g, &h));
+// res (all but gpu_ms, when given) <- the LM scalars at the end of a solve; a non-finite final cost is an error
+static int ba_fill_result(gb_ctx* ctx, const BaScalars& h, gb_ba_result* res) {
   if (res) {
     res->initial_cost = h.initial_cost;
     res->final_cost = h.cost;
@@ -2486,6 +2209,14 @@ int gb_ba_graph_finish(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* res) {
   return GB_OK;
 }
 
+int gb_ba_graph_finish(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* res) {
+  if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
+  CtxLock lk(ctx);
+  BaScalars h;
+  GB_CHECK(ba_read_scalars(ctx, g, &h));
+  return ba_fill_result(ctx, h, res);
+}
+
 // LM loop of a whole solve, then ONE synchronisation for everything the host wants back: the LM scalars and, for the one-shot
 // host-buffer paths, the final T_wc poses / points (pose_out / pts_out may be null).
 static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt, gb_ba_result* res, double* pose_out, double* pts_out) {
@@ -2494,10 +2225,10 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
   GB_CUDA(ctx, cudaEventRecord(ctx->evs, ctx->stream));
   const bool poll = g->opt.function_tolerance > 0.0 || g->opt.verbose;
-  // one fused commit kernel while the estimate fits a single CTA's copy loop; the stepwise kernels otherwise
-  const bool fused_commit = g->d.npe == 0 && (size_t)g->d.np * 3 + (size_t)g->d.nc * 19 <= (size_t)1 << 16;
-  // local-BA fast path (block-CSR Schur + single-CTA PCG): 4 launches per LM iteration
-  const bool local4 = fused_commit && g->pcg_sparse && g->d.s_nnzb > 0 && g->d.nc > 0 && g->d.np > 0;
+  // local-BA fast path (block-CSR Schur + single-CTA PCG): 4 launches per LM iteration, for graphs whose estimate fits the
+  // single-CTA loops of its tail (ba_backsub_commit_kernel's last CTA, ba_install_pending_kernel)
+  const bool local4 = g->d.npe == 0 && (size_t)g->d.np * 3 + (size_t)g->d.nc * 19 <= (size_t)1 << 16 && g->pcg_sparse &&
+                      g->d.s_nnzb > 0 && g->d.nc > 0 && g->d.np > 0;
   for (int it = 0; it < g->opt.max_iterations; ++it) {
     if (local4) {
       BaDev& d = g->d;
@@ -2506,28 +2237,15 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
       // (programmatic dependent launches: each kernel is scheduled while its predecessor drains)
       GB_CUDA(ctx, gb_launch_pdl(ba_linearize_kernel, dim3(pt_blocks + cam_blocks), dim3(kPtThreads), 0, s, d, cam_blocks)); GB_LAUNCH_CHECK(ctx);
       GB_CUDA(ctx, gb_launch_pdl(ba_schur_blocks_kernel, dim3(d.s_nupper), dim3(128), 0, s, d, g->buf)); GB_LAUNCH_CHECK(ctx);
-      if (g->opt.linear_solver == 1) {
-        GB_CHECK(ba_chol_launch(ctx, g, g->buf, true));
-      } else {
-        if (g->pcg_nact <= kSpSmallCams) GB_CUDA(ctx, gb_launch_pdl(BA_SPARSE_SMALL, dim3(1), dim3(kSpSmallThreads), g->pcg_sparse_smem, s, d, g->buf, (int)g->opt.pcg_max_iters));
-        else GB_CUDA(ctx, gb_launch_pdl(BA_SPARSE_LARGE, dim3(1), dim3(kSpLargeThreads), g->pcg_sparse_smem, s, d, g->buf, (int)g->opt.pcg_max_iters));
-        GB_LAUNCH_CHECK(ctx);
-      }
+      if (g->opt.linear_solver == 1) GB_CHECK(ba_chol_launch(ctx, g, g->buf, true));
+      else GB_CHECK(ba_pcg_sparse_launch(ctx, g, g->buf, true));
       GB_CUDA(ctx, gb_launch_pdl(ba_backsub_commit_kernel, dim3(gb_div_up(d.np * kLpp, kTailThreads)), dim3(kTailThreads), 0, s, d, (const double*)g->buf)); GB_LAUNCH_CHECK(ctx);
     } else if (g->pcg_bcsr && g->opt.linear_solver == 0) {  // large graph: compact block-CSR reduced system + the persistent multi-CTA PCG
-      GB_CHECK(ba_reduce_local_compact(ctx, g, g->rbuf));
-      GB_CHECK(ba_pcg_bcsr_launch(ctx, g, g->rbuf));
-      GB_CHECK(ba_backsub_cost_compact(ctx, g, nullptr));
-      GB_CHECK(ba_commit_compact(ctx, g, g->rbuf, nullptr));
-    } else {
-    GB_CHECK(gb_ba_graph_reduce_local(ctx, g, nullptr));
-    if (fused_commit) {
-      GB_CHECK(ba_step_core(ctx, g, g->buf));
-      ba_commit_fused_kernel<<<1, kRedThreads, 0, ctx->stream>>>(g->d, g->buf); GB_LAUNCH_CHECK(ctx);
-    } else {
+      GB_CHECK(ba_compact_iteration(ctx, g, nullptr));
+    } else {  // the stepwise interface on the dense reduced layout
+      GB_CHECK(gb_ba_graph_reduce_local(ctx, g, nullptr));
       GB_CHECK(gb_ba_graph_step(ctx, g, nullptr, nullptr));
       GB_CHECK(gb_ba_graph_commit(ctx, g, nullptr, nullptr));
-    }
     }
     if (poll) {
       BaScalars h;
@@ -2554,21 +2272,8 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   }
   if (hx) GB_CUDA(ctx, cudaMemcpyAsync(hx, dd.pts, bx, cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  const BaScalars& h = *hs;
-  if (res) {
-    res->initial_cost = h.initial_cost;
-    res->final_cost = h.cost;
-    res->iterations = h.iterations;
-    res->accepted = h.accepted;
-    res->pcg_iterations = h.pcg_iters;
-    res->status = h.status;
-    res->lambda_final = h.lambda;
-    GB_CUDA(ctx, cudaEventElapsedTime(&res->gpu_ms, ctx->evs, ctx->eve));
-  }
-  if (!std::isfinite(h.cost)) {
-    gb_set_error(ctx, "gb_ba: non-finite cost");
-    return GB_ERR_NUMERIC;
-  }
+  if (res) GB_CUDA(ctx, cudaEventElapsedTime(&res->gpu_ms, ctx->evs, ctx->eve));
+  GB_CHECK(ba_fill_result(ctx, *hs, res));
   if (hp) memcpy(pose_out, hp, bp);
   if (hx) memcpy(pts_out, hx, bx);
   return GB_OK;

@@ -89,7 +89,7 @@ __global__ void __launch_bounds__(kCholThreads, 1) ba_chol_kernel(BaDev g, doubl
     double v = g.Sb[w];
     if (c == i && (k % 7) == 0) {
       const int comp = k / 7, d = 6 * i + comp;
-      v = ((g.dof[i] >> comp) & 1) ? v + lambda * clampd(buf[nS + n6 + d]) : 1.0;
+      v = lm_damp(v, buf[nS + n6 + d], lambda, (g.dof[i] >> comp) & 1);
     }
     L[(size_t)(rowoff[i] + c - first[i]) * 36 + k] = v;
   }
@@ -202,22 +202,7 @@ __global__ void __launch_bounds__(kCholThreads, 1) ba_chol_kernel(BaDev g, doubl
     g.x[d] = v;
   }
   __syncthreads();
-  for (int i = tid; i < nc; i += kCholThreads) {
-    double pose[7], dd[6], out[7], R[9];
-    const int dm = g.dof[i];
-#pragma unroll
-    for (int k = 0; k < 7; ++k) pose[k] = g.pose[7 * i + k];
-#pragma unroll
-    for (int q = 0; q < 6; ++q) dd[q] = ((dm >> q) & 1) ? y[6 * i + q] : 0.0;
-    se3_retract(pose, dd, out);
-#pragma unroll
-    for (int k = 0; k < 7; ++k) g.pose_new[7 * i + k] = out[k];
-    quat_to_R(out, R);
-#pragma unroll
-    for (int k = 0; k < 9; ++k) g.Rt_new[12 * i + k] = R[k];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) g.Rt_new[12 * i + 9 + k] = out[4 + k];
-  }
+  for (int i = tid; i < nc; i += kCholThreads) retract_camera(g, i, y + 6 * i);
 }
 
 }  // namespace

@@ -16,8 +16,8 @@ struct BaScalars {
   // PCG state (generic multi-kernel path): gamma = r'u, gamma0 its initial value, CG step sizes
   double rz, rz0, pcg_alpha, pcg_beta;
   int pcg_first, pcg_k;
-  int need_linearize, stop, status, iterations, accepted, accept_flag;
-  unsigned int ticket;  // last-CTA-done counter of the fused back-substitution + commit kernel
+  int need_linearize, stop, status, iterations, accepted;
+  unsigned int ticket;  // last-CTA-done counter of the fused back-substitution + commit kernel (ba_backsub_commit_kernel)
   int pending;          // an accepted candidate (pose_new / Rt_new / pts_new) has not been installed yet: the next sweep reads the
                         // candidate arrays and installs them on the fly (ba_install_pending_kernel at the end of a solve)
   int pcg_iters, pcg_done;
@@ -176,6 +176,87 @@ __device__ __forceinline__ bool spd_inverse(double* A) {
       A[i * N + j] = s;
     }
   return true;
+}
+
+// ---- the rules of the Levenberg-Marquardt step, each written once for every solver path -----------------------------------------
+
+// LM accept / reject of a step from the cost at the current estimate and at the candidate (one thread).  Accept: lambda / 3 floored
+// at 1e-15, nu = 2, stop with status 1 when the relative decrease is under ftol.  Reject: lambda * nu, nu * 2, stop with status 2
+// once lambda exceeds 1e16.  Returns whether the step was accepted: lm_accepts, which any thread may evaluate from the two costs.
+__device__ __forceinline__ bool lm_accepts(double cost, double cnew) { return (cnew < cost) && isfinite(cnew); }
+__device__ __forceinline__ bool lm_decide(BaScalars* sc, double cost, double cnew) {
+  if (sc->iterations == 0) sc->initial_cost = cost;
+  sc->cost = cost;
+  sc->cost_new = cnew;
+  sc->iterations++;
+  const bool ok = lm_accepts(cost, cnew);
+  sc->need_linearize = ok ? 1 : 0;
+  if (ok) {
+    const double rel = (cost - cnew) / cost;
+    sc->cost = cnew;
+    const double l = sc->lambda / 3.0;
+    sc->lambda = l < 1e-15 ? 1e-15 : l;
+    sc->nu = 2.0;
+    sc->accepted++;
+    if (rel < sc->ftol) { sc->stop = 1; sc->status = 1; }
+  } else {
+    sc->lambda *= sc->nu;
+    sc->nu *= 2.0;
+    if (sc->lambda > 1e16) { sc->stop = 1; sc->status = 2; }
+  }
+  return ok;
+}
+
+// Marquardt damping of the diagonal entry s of a normal-equation block whose undamped value is diag; a fixed dof gets a unit diagonal
+__device__ __forceinline__ double lm_damp(double s, double diag, double lambda, bool free = true) {
+  return free ? s + lambda * clampd(diag) : 1.0;
+}
+
+// Block-Jacobi preconditioner block: M (a damped 6x6 diagonal block, read from D with row stride ld) <- its inverse, or the inverse
+// of its diagonal when the block is not positive definite
+__device__ __forceinline__ void block_jacobi_inverse(double* M, const double* D, size_t ld) {
+  if (!spd_inverse<6>(M)) {
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+#pragma unroll
+      for (int b = 0; b < 6; ++b) M[a * 6 + b] = (a == b) ? 1.0 / D[a * ld + a] : 0.0;
+  }
+}
+
+// Damped landmark inverse: Vinv[9] = (V + lambda * clamp(diag V))^-1 for an active landmark (free and observed); zero when the
+// landmark is not active or the damped block is not positive definite
+__device__ __forceinline__ void damped_vinv(const double* V, bool active, double lambda, double* Vinv) {
+  double Vi[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) Vi[k] = active ? V[k] : 0.0;
+  if (active) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) Vi[a * 4] = lm_damp(Vi[a * 4], Vi[a * 4], lambda);
+    if (!spd_inverse<3>(Vi)) {
+#pragma unroll
+      for (int k = 0; k < 9; ++k) Vi[k] = 0.0;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 9; ++k) Vinv[k] = Vi[k];
+}
+
+// Candidate of camera i: pose_new = Exp(dx) * pose and its Rt_new, with dx[6] restricted to the camera's free dofs
+__device__ __forceinline__ void retract_camera(const BaDev& g, int i, const double* dx) {
+  double pose[7], d[6], out[7], R[9];
+  const int dm = g.dof[i];
+#pragma unroll
+  for (int k = 0; k < 7; ++k) pose[k] = g.pose[7 * i + k];
+#pragma unroll
+  for (int a = 0; a < 6; ++a) d[a] = ((dm >> a) & 1) ? dx[a] : 0.0;
+  se3_retract(pose, d, out);
+#pragma unroll
+  for (int k = 0; k < 7; ++k) g.pose_new[7 * i + k] = out[k];
+  quat_to_R(out, R);
+#pragma unroll
+  for (int k = 0; k < 9; ++k) g.Rt_new[12 * i + k] = R[k];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) g.Rt_new[12 * i + 9 + k] = out[4 + k];
 }
 
 struct ObsLin {

@@ -185,12 +185,7 @@ int gb_ba_shard_solve(gb_comm* c, gb_ba_graph* g, const gb_ba_options* opt, gb_b
   GB_CUDA(ctx, cudaEventRecord(ctx->evs, ctx->stream));
   const bool poll = g->opt.function_tolerance > 0.0 || g->opt.verbose;
   for (int it = 0; it < g->opt.max_iterations; ++it) {
-    GB_CHECK(ba_reduce_local_compact(ctx, g, g->rbuf));
-    GB_CHECK(gb_comm_allreduce_sum_f64(c, g->rbuf, g->rbuf_doubles));
-    GB_CHECK(ba_pcg_bcsr_launch(ctx, g, g->rbuf));
-    GB_CHECK(ba_backsub_cost_compact(ctx, g, g->d_cost));
-    GB_CHECK(gb_comm_allreduce_sum_f64(c, g->d_cost, 1));
-    GB_CHECK(ba_commit_compact(ctx, g, g->rbuf, g->d_cost));
+    GB_CHECK(ba_compact_iteration(ctx, g, c));
     if (poll) {  // every rank reads the same (reduced) scalars, so every rank stops at the same iteration
       BaScalars h;
       GB_CUDA(ctx, cudaMemcpyAsync(&h, g->d.sc, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
@@ -202,7 +197,7 @@ int gb_ba_shard_solve(gb_comm* c, gb_ba_graph* g, const gb_ba_options* opt, gb_b
     }
   }
   GB_CUDA(ctx, cudaEventRecord(ctx->eve, ctx->stream));
-  GB_CHECK(ba_read_result(ctx, g, res));
+  GB_CHECK(gb_ba_graph_finish(ctx, g, res));
   if (res) GB_CUDA(ctx, cudaEventElapsedTime(&res->gpu_ms, ctx->evs, ctx->eve));
   return GB_OK;
 }

@@ -60,11 +60,10 @@ struct gb_ba_graph {
 // all cameras and the GLOBAL covisibility block structure are kept, so that every rank's reduced system has the same layout.
 int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out, bool use_arena, int shard_rank, int shard_world,
                          const gb_pose_edges* pose_edges = nullptr);
-// one LM iteration in pieces, on the COMPACT reduced layout rbuf = [Sb | g~ | diag U | cost | pad] (g->rbuf_doubles doubles):
-int ba_reduce_local_compact(gb_ctx* ctx, gb_ba_graph* g, double* rbuf);           // sweep (if needed) + Schur blocks of the shard
-int ba_backsub_cost_compact(gb_ctx* ctx, gb_ba_graph* g, double* d_cost);         // back-substitution + candidate cost of the shard
-int ba_commit_compact(gb_ctx* ctx, gb_ba_graph* g, const double* rbuf, const double* d_cost);  // LM accept / reject + install
-int ba_read_result(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* res);               // one sync; fills res from the device scalars
+// one LM iteration on the COMPACT reduced layout g->rbuf = [Sb | g~ | diag U | cost | pad] (g->rbuf_doubles doubles): sweep (if
+// needed) + Schur blocks, block-CSR PCG, back-substitution + candidate cost, LM accept / reject + install.  A non-null `comm`
+// all-reduces the reduced system and the candidate cost of this landmark shard before they are used.
+int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
 
 // ---- ba_pose.cu -------------------------------------------------------------------------------------------------------------
 // pose-graph terms (SE3Edge / GPSEdge, Optimizer.h:127-148) on the stepwise dense-layout solver path

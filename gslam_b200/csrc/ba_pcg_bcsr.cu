@@ -106,7 +106,7 @@ __global__ void __launch_bounds__(kBcsrThreads, 1) ba_pcg_bcsr_kernel(BaDev g, d
     if (diag >= 0) {
       double* e = (a.in_smem ? Ssm + (size_t)diag * a.blk_stride : Sg + (size_t)diag * 36) + comp * 7;
       const double du = __ldcg(rbuf + r_gt + n6 + 6 * cam + comp);
-      *e = ((g.dof[cam] >> comp) & 1) ? *e + lambda * clampd(du) : 1.0;
+      *e = lm_damp(*e, du, lambda, (g.dof[cam] >> comp) & 1);
     }
   }
   __syncthreads();
@@ -119,10 +119,7 @@ __global__ void __launch_bounds__(kBcsrThreads, 1) ba_pcg_bcsr_kernel(BaDev g, d
     double M[36];
 #pragma unroll
     for (int k = 0; k < 36; ++k) M[k] = D[k];
-    if (!spd_inverse<6>(M)) {
-#pragma unroll
-      for (int k = 0; k < 36; ++k) M[k] = (k % 7 == 0) ? 1.0 / D[k] : 0.0;
-    }
+    block_jacobi_inverse(M, D, 6);
 #pragma unroll
     for (int k = 0; k < 36; ++k) Minv[36 * c + k] = M[k];
   }
@@ -301,22 +298,7 @@ __global__ void __launch_bounds__(kBcsrThreads, 1) ba_pcg_bcsr_kernel(BaDev g, d
   }
   // ---- F. solution + retraction of the owned cameras ----
   for (int r = tid; r < rows; r += kBcsrThreads) g.x[6 * cam0 + r] = vx[r];
-  for (int c = tid; c < ncl; c += kBcsrThreads) {
-    const int i = cam0 + c, dm = g.dof[i];
-    double pose[7], d[6], out[7], R[9];
-#pragma unroll
-    for (int k = 0; k < 7; ++k) pose[k] = g.pose[7 * i + k];
-#pragma unroll
-    for (int q = 0; q < 6; ++q) d[q] = ((dm >> q) & 1) ? vx[6 * c + q] : 0.0;
-    se3_retract(pose, d, out);
-#pragma unroll
-    for (int k = 0; k < 7; ++k) g.pose_new[7 * i + k] = out[k];
-    quat_to_R(out, R);
-#pragma unroll
-    for (int k = 0; k < 9; ++k) g.Rt_new[12 * i + k] = R[k];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) g.Rt_new[12 * i + 9 + k] = out[4 + k];
-  }
+  for (int c = tid; c < ncl; c += kBcsrThreads) retract_camera(g, cam0 + c, vx + 6 * c);
   if (b == 0 && tid == 0) g.sc->pcg_iters += k_it;
   if (CLUSTER) cg::this_cluster().sync();  // nobody leaves while a peer could still address its shared memory
 }

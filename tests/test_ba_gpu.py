@@ -447,3 +447,29 @@ def test_host_buffer_solve_topology_cache(ctx, monkeypatch):
         q = p.copy(); r = ctx.ba_solve(q, c)
         assert r.final_cost == want[0] and r.accepted == want[1]
         assert np.array_equal(q.cam_pose_wc, want[2]) and np.array_equal(q.points, want[3])
+
+
+def test_stepwise_interface_with_caller_buffers_matches_solve(ctx):
+    """gb_ba_graph_begin, then per LM iteration reduce_local -> step -> commit on caller-owned device buffers, then finish: the
+    same bits as gb_ba_graph_solve of the same graph (whose dense-layout branch runs exactly these calls)."""
+    import torch
+    pb = synth.synth_ba(**PROBLEMS["local_50kf"])
+    c = cfg(maxIterations=6, functionTolerance=0.0)
+    g = BAGraph(ctx, pb)
+    g.force_generic_pcg(1)  # off the local-BA launch chain, onto the dense reduced layout
+    want = g.solve(c); p0, x0 = g.download()
+    g.reset()
+    buf = torch.zeros(g.reduce_size(), dtype=torch.float64, device="cuda")
+    cost = torch.zeros(1, dtype=torch.float64, device="cuda")
+    torch.cuda.synchronize()  # (the library works on its own stream)
+    g.begin(c)
+    for _ in range(c.maxIterations):
+        g.reduce_local(buf.data_ptr())
+        g.step(buf.data_ptr(), cost.data_ptr())
+        g.commit(buf.data_ptr(), cost.data_ptr())
+    got = g.finish(); p1, x1 = g.download()
+    g.close()
+    assert 0 < got.accepted and got.iterations == want.iterations == c.maxIterations
+    for f in ("initial_cost", "final_cost", "accepted", "pcg_iterations", "status", "lambda_final"):
+        assert getattr(got, f) == getattr(want, f), f
+    assert np.array_equal(p1, p0) and np.array_equal(x1, x0)
