@@ -432,6 +432,16 @@ class BAGraph:
     def pcg_cluster_size(self) -> int:
         return int(self.ctx._lib.gb_dbg_ba_pcg_cluster_size(self.ctx._h, self._h))
 
+    # bits of paths(): what a solve of this graph would run, as planned now (gb_dbg_ba_paths in csrc/ba.cu)
+    LOCAL4, PCG_SPARSE, PCG_CLUSTER, PCG_BCSR, BCSR_CLUSTER, SCHUR_CHUNKS, SWEEP_LARGE, DENSE_ATOMIC, CHOL_OK, CAM_SPLIT = (1 << k for k in range(10))
+
+    def paths(self) -> int:
+        """Bitmask of the solver paths (test hook): see the BAGraph.LOCAL4 ... CAM_SPLIT constants."""
+        v = int(self.ctx._lib.gb_dbg_ba_paths(self.ctx._h, self._h))
+        if v < 0:
+            raise GbError(v, "gb_dbg_ba_paths")
+        return v
+
     def dbg_reduced(self, cfg: OptimzeConfig | None = None):
         n6 = 6 * self.n_cams
         S = np.zeros((n6, n6)); gt = np.zeros(n6); dc = np.zeros(n6); it = C.c_int()

@@ -134,6 +134,7 @@ _DEBUG_SIGNATURES = [
     ("gb_dbg_ba_force_generic_pcg", C.c_int, [_VP, _VP, C.c_int]),
     ("gb_dbg_ba_pcg_cluster_size", C.c_int, [_VP, _VP]),
     ("gb_dbg_ba_pcg_sparse", C.c_int, [_VP, _VP]),
+    ("gb_dbg_ba_paths", C.c_int, [_VP, _VP]),
     ("gb_dbg_ba_set_cam_split", C.c_int, [_VP, _VP, C.c_int]),
     ("gb_dbg_ba_sweep_part", C.c_int, [_VP, _VP, C.c_int]),
     ("gb_dbg_ba_set_sweep", C.c_int, [_VP, _VP, C.c_int]),

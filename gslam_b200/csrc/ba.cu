@@ -2077,7 +2077,7 @@ int gb_ba_graph_reduce_local(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
   d.vinv_in_sweep = ba_sweep_is_large(g) ? 0 : 1;
   GB_CHECK(ba_launch_sweep(ctx, g, d, s, 3));
   GB_CHECK(ba_pose_linearize(ctx, g, s));  // (pose-graph terms, if any: into U, g_c and the cost terms before they are consumed)
-  // Schur complement.  With the covisibility block structure at hand (<= 1024 cameras) S is formed block by block without
+  // Schur complement.  With the covisibility block structure at hand (<= kMaxBlockCams = 2048 cameras) S is formed block by block without
   // atomics (deterministic); the local-BA solver consumes the block-CSR directly, every other consumer (one-cluster / generic
   // PCG, the multi-GPU all-reduce) gets it scattered into the dense layout of `buf`.
   const bool have_blocks = d.s_nnzb > 0 && d.nc > 0;
@@ -2217,6 +2217,13 @@ int gb_ba_graph_finish(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* res) {
   return ba_fill_result(ctx, h, res);
 }
 
+// local-BA fast path (block-CSR Schur + single-CTA PCG): 4 launches per LM iteration, for graphs whose estimate fits the
+// single-CTA loops of its tail (ba_backsub_commit_kernel's last CTA, ba_install_pending_kernel)
+static bool ba_takes_local4(const gb_ba_graph* g) {
+  return g->d.npe == 0 && (size_t)g->d.np * 3 + (size_t)g->d.nc * 19 <= (size_t)1 << 16 && g->pcg_sparse && g->d.s_nnzb > 0 && g->d.nc > 0 &&
+         g->d.np > 0;
+}
+
 // LM loop of a whole solve, then ONE synchronisation for everything the host wants back: the LM scalars and, for the one-shot
 // host-buffer paths, the final T_wc poses / points (pose_out / pts_out may be null).
 static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt, gb_ba_result* res, double* pose_out, double* pts_out) {
@@ -2225,10 +2232,7 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
   GB_CUDA(ctx, cudaEventRecord(ctx->evs, ctx->stream));
   const bool poll = g->opt.function_tolerance > 0.0 || g->opt.verbose;
-  // local-BA fast path (block-CSR Schur + single-CTA PCG): 4 launches per LM iteration, for graphs whose estimate fits the
-  // single-CTA loops of its tail (ba_backsub_commit_kernel's last CTA, ba_install_pending_kernel)
-  const bool local4 = g->d.npe == 0 && (size_t)g->d.np * 3 + (size_t)g->d.nc * 19 <= (size_t)1 << 16 && g->pcg_sparse &&
-                      g->d.s_nnzb > 0 && g->d.nc > 0 && g->d.np > 0;
+  const bool local4 = ba_takes_local4(g);
   for (int it = 0; it < g->opt.max_iterations; ++it) {
     if (local4) {
       BaDev& d = g->d;
@@ -2557,6 +2561,20 @@ GB_API int gb_dbg_ba_set_sweep(gb_ctx* ctx, gb_ba_graph* g, int mode) {
 }
 
 GB_API int gb_dbg_ba_pcg_cluster_size(gb_ctx* ctx, gb_ba_graph* g) { return (ctx && g) ? g->pcg_cluster : -1; }
+
+// What a solve of this graph would run, as it is planned now (after any of the hooks above), one bit per host-side decision:
+//   1 local4: the 4-launch local-BA chain          2 pcg_sparse: single-CTA block-sparse PCG    4 one-cluster PCG (pcg_cluster > 0)
+//   8 pcg_bcsr: compact block-CSR PCG               16 ... in one thread-block cluster (else as a cooperative grid)
+//   32 landmark-chunk Schur plan (else block gather)   64 persistent large-graph sweep (ba_sweep.cu)
+//   128 no block structure: dense Schur by fp64 atomics   256 chol_ok: the direct solver fits   512 camera pass sliced (cam_split > 1)
+// Tests assert these bits so that a threshold change cannot quietly turn one path's test into a duplicate of another's.
+GB_API int gb_dbg_ba_paths(gb_ctx* ctx, gb_ba_graph* g) {
+  if (!ctx || !g) return -1;
+  const BaDev& d = g->d;
+  return (ba_takes_local4(g) ? 1 : 0) | (g->pcg_sparse ? 2 : 0) | (g->pcg_cluster > 0 ? 4 : 0) | (g->pcg_bcsr ? 8 : 0) |
+         (g->pcg_bcsr && g->bcsr_cluster > 0 ? 16 : 0) | (d.sp_nchunks > 0 ? 32 : 0) | (ba_sweep_is_large(g) ? 64 : 0) |
+         (d.s_nnzb == 0 && d.nc > 0 ? 128 : 0) | (g->chol_ok ? 256 : 0) | (d.cam_split > 1 ? 512 : 0);
+}
 
 // clock64 stamps of PCG iteration 3 on CTA 0 (8 values): enable, solve, then read
 GB_API int gb_dbg_ba_pcg_profile(gb_ctx* ctx, gb_ba_graph* g, long long* out8) {

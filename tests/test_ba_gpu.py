@@ -365,6 +365,9 @@ def test_large_graph_paths_agree_and_match_oracle(ctx, monkeypatch):
     want = pb0.copy()
     r0 = oracle.ba_solve(want, max_iterations=5, function_tolerance=0.0, pcg_max_iters=600)
     results = {}
+    # the plans are made at graph creation: without this the host-buffer solve's topology cache would hand every variant the
+    # graph (and the plan) of the first
+    monkeypatch.setenv("GB_BA_NO_CACHE", "1")
     for name, env in (("chunks+cluster", {}), ("gather+cluster", {"GB_BA_NO_SCHUR_CHUNKS": "1"}), ("chunks+grid", {"GB_BA_NO_PCG_CLUSTER": "1"})):
         for k in ("GB_BA_NO_SCHUR_CHUNKS", "GB_BA_NO_PCG_CLUSTER"):
             monkeypatch.delenv(k, raising=False)

@@ -20,6 +20,7 @@ import scipy.sparse.linalg as spla
 
 import oracle
 from gslam_b200 import synth
+import ba_graphs  # (tests/ is on sys.path under pytest's rootdir conftest)
 
 
 def quat_to_R(q):
@@ -170,10 +171,14 @@ def _variant(kind):
         pb.cam_dof[2] = 0b000111          # translation only
         pb.point_free[::7] = 0            # some fixed landmarks
         return pb, 0.01
+    if kind in ba_graphs.CASES:           # the irregular topologies of tests/ba_graphs.py, local-window size
+        c = ba_graphs.build(kind)
+        return c.pb, c.delta
     raise KeyError(kind)
 
 
-@pytest.mark.parametrize("kind,iters", [("config1_huber", 8), ("local_window_huber", 6), ("info_and_partial_dof", 8)])
+@pytest.mark.parametrize("kind,iters", [("config1_huber", 8), ("local_window_huber", 6), ("info_and_partial_dof", 8)] +
+                         [(name, 6) for name in ba_graphs.CASES])
 def test_oracle_lm_trajectory_equals_independent_sparse_lm(kind, iters):
     pb, delta = _variant(kind)
     trace, accepted, t_wc, pts = lm_numpy(pb, iters, delta)
