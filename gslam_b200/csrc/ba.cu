@@ -1371,16 +1371,37 @@ static size_t ba_buf_doubles(int nc) {
   return n6 * n6 + 2 * n6 + 8;
 }
 
-struct Slab {
-  uint8_t* base = nullptr;
-  size_t off = 0;
-  template <typename T>
-  void take(T** p, size_t n) {
-    off = (off + 255) & ~(size_t)255;
-    if (base) *p = (T*)(base + off);
-    off += std::max<size_t>(n, 1) * sizeof(T);
+// a measurement's x and y are divided by its z (graph creation and the refresh of a cached graph)
+static int ba_check_z(gb_ctx* ctx, const gb_ba_problem* pb, int k) {
+  const double z = pb->obs_xyz[3 * (size_t)k + 2];
+  if (!(z != 0.0) || !std::isfinite(z)) {
+    gb_set_error(ctx, "gb_ba: edge %d has a zero/non-finite measurement z", k);
+    return GB_ERR_INVALID;
   }
-};
+  return GB_OK;
+}
+
+// the measurements as the kernels read them: x/z, y/z in sorted edge order (uv) and in camera order (cuv), and the symmetrised 2x2
+// information in sorted order (info, when the problem has it).  sorted_to_orig and cam_perm as in gb_ba_graph.
+static void ba_fill_measurements(const gb_ba_problem* pb, const std::vector<int>& sorted_to_orig, const std::vector<int>& cam_perm, double* uv,
+                                 double* cuv, double* info) {
+  const size_t no = sorted_to_orig.size();
+  for (size_t e = 0; e < no; ++e) {
+    const int k = sorted_to_orig[e];
+    const double* m = pb->obs_xyz + 3 * (size_t)k;
+    uv[2 * e] = m[0] / m[2];
+    uv[2 * e + 1] = m[1] / m[2];
+    if (info) {
+      const double* L = pb->obs_info + 4 * (size_t)k;
+      info[3 * e] = L[0]; info[3 * e + 1] = 0.5 * (L[1] + L[2]); info[3 * e + 2] = L[3];
+    }
+  }
+  for (size_t idx = 0; idx < no; ++idx) {
+    const int e = cam_perm[idx];
+    cuv[2 * idx] = uv[2 * e];
+    cuv[2 * idx + 1] = uv[2 * e + 1];
+  }
+}
 
 static int ba_validate(gb_ctx* ctx, const gb_ba_problem* pb) {
   if (!pb || pb->n_cams < 0 || pb->n_points < 0 || pb->n_obs < 0) {
@@ -1401,40 +1422,9 @@ static int ba_validate(gb_ctx* ctx, const gb_ba_problem* pb) {
       gb_set_error(ctx, "gb_ba: edge %d references camera %d / point %d out of range", k, pb->obs_cam[k], pb->obs_point[k]);
       return GB_ERR_INVALID;
     }
-    const double z = pb->obs_xyz[3 * (size_t)k + 2];
-    if (!(z != 0.0) || !std::isfinite(z)) {
-      gb_set_error(ctx, "gb_ba: edge %d has a zero/non-finite measurement z", k);
-      return GB_ERR_INVALID;
-    }
+    GB_CHECK(ba_check_z(ctx, pb, k));
   }
   return GB_OK;
-}
-
-// The dynamic shared-memory limit of a kernel is per-function, per-DEVICE global state: raise it ONCE per device to the opt-in
-// maximum and never lower it -- several ctxs (tracking thread: gb_ba_pnp on a 1-camera graph; mapping thread: local BA) share
-// the functions, and a per-graph value set by one could be too small for a launch already planned by the other.
-static bool g_cluster16_ok[64] = {false};
-static bool ba_raise_smem_limits(gb_ctx* ctx) {
-  static std::mutex mu;
-  static int state[64] = {0};  // 0 = not done, 1 = ok, 2 = failed
-  const int dev = ctx->device;
-  if (dev < 0 || dev >= 64) return false;
-  std::lock_guard<std::mutex> lk(mu);
-  if (state[dev] == 0) {
-    g_cluster16_ok[dev] = cudaFuncSetAttribute(ba_pcg_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
-    // (the opt-in maximum covers static + dynamic shared memory: leave room for each kernel's static part)
-    auto raise = [&](const void* fn) {
-      cudaFuncAttributes fa;
-      if (cudaFuncGetAttributes(&fa, fn) != cudaSuccess) return false;
-      return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->max_smem_optin - (int)fa.sharedSizeBytes) == cudaSuccess;
-    };
-    bool ok = raise((const void*)BA_SPARSE_SMALL);
-    ok = raise((const void*)BA_SPARSE_LARGE) && ok;
-    ok = raise((const void*)ba_pcg_cluster_kernel) && ok;
-    cudaGetLastError();
-    state[dev] = ok ? 1 : 2;
-  }
-  return state[dev] == 1;
 }
 
 // Can the reduced camera system be solved by the one-cluster PCG kernel?  Pick the cluster size, remember the smem need.
@@ -1442,7 +1432,10 @@ static void ba_pick_pcg(gb_ctx* ctx, gb_ba_graph* g) {
   g->pcg_cluster = 0;
   g->pcg_sparse = false;
   const int nc = g->d.nc, n6 = g->d.n6;
-  const bool smem_ok = ba_raise_smem_limits(ctx);
+  bool cluster16_ok = false;
+  bool smem_ok = gb_func_setup(ctx, (const void*)BA_SPARSE_SMALL, GB_SMEM_OPTIN_MAX);
+  smem_ok = gb_func_setup(ctx, (const void*)BA_SPARSE_LARGE, GB_SMEM_OPTIN_MAX) && smem_ok;
+  smem_ok = gb_func_setup(ctx, (const void*)ba_pcg_cluster_kernel, GB_SMEM_OPTIN_MAX, &cluster16_ok) && smem_ok;
   if (nc > 0 && g->pcg_nact <= kSpMaxCams && g->d.s_nnzb > 0) {
     const size_t smem = ((size_t)g->d.s_nnzb * 36 + (size_t)nc * 36 + 3 * (size_t)n6) * sizeof(double) + (2 * (size_t)nc + 1 + g->d.s_nnzb) * sizeof(int) + 64;
     if (smem + 2048 <= (size_t)ctx->max_smem_optin && smem_ok) {
@@ -1451,7 +1444,7 @@ static void ba_pick_pcg(gb_ctx* ctx, gb_ba_graph* g) {
     }
   }
   if (nc <= 0 || n6 > kPcgThreads) return;  // the cluster kernel maps one thread per element of the 6N vectors
-  const bool np_ok = smem_ok && g_cluster16_ok[ctx->device];
+  const bool np_ok = smem_ok && cluster16_ok;
   const int sizes[2] = {16, 8};
   for (int t = 0; t < 2; ++t) {
     const int C = sizes[t];
@@ -1459,14 +1452,9 @@ static void ba_pick_pcg(gb_ctx* ctx, gb_ba_graph* g) {
     const int cpc = (nc + C - 1) / C;
     const size_t smem = ((size_t)6 * cpc * n6 + (size_t)nc * 36 + 7 * (size_t)n6) * sizeof(double) + 64;
     if (smem + 2048 > (size_t)ctx->max_smem_optin || !smem_ok) continue;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(C); cfg.blockDim = dim3(kPcgThreads); cfg.dynamicSmemBytes = smem; cfg.stream = ctx->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
+    GbClusterConfig lc(C, dim3(kPcgThreads), smem, ctx->stream);
     int nclusters = 0;
-    if (cudaOccupancyMaxActiveClusters(&nclusters, ba_pcg_cluster_kernel, &cfg) != cudaSuccess || nclusters < 1) {
+    if (cudaOccupancyMaxActiveClusters(&nclusters, ba_pcg_cluster_kernel, &lc.cfg) != cudaSuccess || nclusters < 1) {
       cudaGetLastError();
       continue;
     }
@@ -1507,21 +1495,15 @@ void gb_ba_options_default(gb_ba_options* o) {
 
 int gb_ba_graph_destroy(gb_ctx* ctx, gb_ba_graph* g) {
   if (!g) return GB_OK;
-  if (g->bcsr_cta_cam || g->sp_alloc || g->sw_alloc || g->pe_alloc) {
-    if (ctx) { CtxLock lk(ctx); cudaStreamSynchronize(ctx->stream); }
-    if (g->bcsr_cta_cam) ba_pcg_bcsr_free(g);
-    if (g->sp_alloc) cudaFree(g->sp_alloc);
-    g->sp_alloc = nullptr;
-    ba_sweep_plan_drop(g);
-    ba_pose_free(g);
+  if (ctx && (!g->from_arena || g->sw_alloc || g->d.prof)) {
+    CtxLock lk(ctx);
+    cudaStreamSynchronize(ctx->stream);
   }
+  ba_sweep_plan_drop(g);
+  cudaFree(g->d.prof);
   if (g->from_arena) {
     if (ctx) ctx->ba_arena_busy = false;
   } else {
-    if (ctx) {
-      CtxLock lk(ctx);
-      cudaStreamSynchronize(ctx->stream);
-    }
     cudaFree(g->slab);
   }
   delete g;
@@ -1539,16 +1521,16 @@ int gb_ba_graph_create_ex(gb_ctx* ctx, const gb_ba_problem* pb, const gb_pose_ed
 
 }  // extern "C"
 
-// Landmark-chunk plan of the Schur complement (see ba_schur_chunks_kernel).  Returns false when it does not apply (a landmark with
-// more than 16 observers, no block structure): the block-gather kernel is used then.
+// Landmark-chunk plan of the Schur complement (see ba_schur_chunks_kernel), host only: sets d.sp_nchunks and fills p.  Returns
+// false when it does not apply (a landmark with more than 16 observers, no block structure): the block-gather kernel is used then.
 static bool ba_schur_plan(gb_ctx* ctx, gb_ba_graph* g, int np, const std::vector<int>& pt_off, const std::vector<int>& scam, const uint8_t* pfree_host,
-                          const std::vector<int>& s_rowptr, const std::vector<int>& s_col, const std::vector<int>& s_upper) {
+                          const std::vector<int>& s_rowptr, const std::vector<int>& s_col, const std::vector<int>& s_upper, BaSchurPlan& p) {
   BaDev& d = g->d;
   d.sp_nchunks = 0;
   if (np <= 0 || d.s_nnzb <= 0 || d.nc <= 0) return false;
   // landmarks in the order of the trajectory (first observing camera, then last, then id): consecutive landmarks then share
   // their cameras whatever order the caller numbered them in; fixed / unobserved landmarks contribute nothing and are left out
-  std::vector<int> ord;
+  std::vector<int>& ord = p.order;
   ord.reserve(np);
   for (int j = 0; j < np; ++j) {
     const int a = pt_off[j], b = pt_off[j + 1];
@@ -1566,8 +1548,9 @@ static bool ba_schur_plan(gb_ctx* ctx, gb_ba_graph* g, int np, const std::vector
   });
   const int nl = (int)ord.size();
   const int lmax = std::min(kChunkMaxLm, std::max(8, nl / (4 * std::max(ctx->sm_count, 1))));
-  std::vector<int> ch_pt0, ch_cams;  // ch_cams: 16 per chunk, ascending, -1 padded
-  std::vector<unsigned short> mask((size_t)nl, 0);
+  std::vector<int> &ch_pt0 = p.pt0, ch_cams;  // ch_cams: 16 per chunk, ascending, -1 padded
+  std::vector<unsigned short>& mask = p.mask;
+  mask.assign((size_t)nl, 0);
   std::vector<int> cur, merged;  // sorted cameras of the open chunk
   int open_from = 0;
   auto close = [&](int upto) {
@@ -1597,8 +1580,10 @@ static bool ba_schur_plan(gb_ctx* ctx, gb_ba_graph* g, int np, const std::vector
   std::vector<std::vector<int>> blk_contrib(s_upper.size()), cam_contrib((size_t)d.nc);
   std::vector<int> upper_of((size_t)d.s_nnzb, -1);
   for (size_t u = 0; u < s_upper.size(); ++u) upper_of[s_upper[u]] = (int)u;
-  std::vector<uint8_t> used(kChunkSlots), slots((size_t)nch * kChunkSlots, 0);
-  std::vector<int> nused((size_t)nch, 0);
+  std::vector<uint8_t> used(kChunkSlots), &slots = p.slots;
+  std::vector<int>& nused = p.nused;
+  slots.assign((size_t)nch * kChunkSlots, 0);
+  nused.assign((size_t)nch, 0);
   for (int c = 0; c < nch; ++c) {
     const int* cams = &ch_cams[(size_t)c * kChunkCams];
     std::fill(used.begin(), used.end(), 0);
@@ -1628,36 +1613,11 @@ static bool ba_schur_plan(gb_ctx* ctx, gb_ba_graph* g, int np, const std::vector
         slots[(size_t)c * kChunkSlots + nused[c]++] = (uint8_t)(lb * (lb + 1) / 2 + la);
       }
   }
-  std::vector<int> boff(s_upper.size() + 1, 0), bidx, coff((size_t)d.nc + 1, 0), cidx;
+  std::vector<int> &boff = p.boff, &bidx = p.bidx, &coff = p.coff, &cidx = p.cidx;
+  boff.assign(s_upper.size() + 1, 0);
+  coff.assign((size_t)d.nc + 1, 0);
   for (size_t u = 0; u < s_upper.size(); ++u) { bidx.insert(bidx.end(), blk_contrib[u].begin(), blk_contrib[u].end()); boff[u + 1] = (int)bidx.size(); }
   for (int i = 0; i < d.nc; ++i) { cidx.insert(cidx.end(), cam_contrib[i].begin(), cam_contrib[i].end()); coff[i + 1] = (int)cidx.size(); }
-  // one device allocation: plan arrays + staging
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t b_pt0 = al((size_t)(nch + 1) * 4), b_mask = al((size_t)nl * 2), b_ord = al((size_t)nl * 4), b_nu = al((size_t)nch * 4), b_sl = al(slots.size()), b_boff = al(boff.size() * 4), b_bidx = al(bidx.size() * 4 + 4),
-               b_coff = al(coff.size() * 4), b_cidx = al(cidx.size() * 4 + 4), b_stS = al((size_t)nch * kChunkSlots * 36 * 8),
-               b_stG = al((size_t)nch * kChunkCams * 6 * 8);
-  uint8_t* base = nullptr;
-  if (cudaMalloc((void**)&base, b_pt0 + b_mask + b_ord + b_nu + b_sl + b_boff + b_bidx + b_coff + b_cidx + b_stS + b_stG) != cudaSuccess) { cudaGetLastError(); return false; }
-  g->sp_alloc = base;
-  size_t off = 0;
-  auto up = [&](const void* src, size_t bytes, size_t padded) {
-    uint8_t* p = base + off;
-    off += padded;
-    if (bytes) cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
-    return p;
-  };
-  d.sp_pt0 = (const int*)up(ch_pt0.data(), (size_t)(nch + 1) * 4, b_pt0);
-  d.sp_mask = (const unsigned short*)up(mask.data(), (size_t)nl * 2, b_mask);
-  d.sp_order = (const int*)up(ord.data(), (size_t)nl * 4, b_ord);
-  d.sp_nused = (const int*)up(nused.data(), (size_t)nch * 4, b_nu);
-  d.sp_slots = (const unsigned char*)up(slots.data(), slots.size(), b_sl);
-  d.sp_boff = (const int*)up(boff.data(), boff.size() * 4, b_boff);
-  d.sp_bidx = (const int*)up(bidx.data(), bidx.size() * 4, b_bidx);
-  d.sp_coff = (const int*)up(coff.data(), coff.size() * 4, b_coff);
-  d.sp_cidx = (const int*)up(cidx.data(), cidx.size() * 4, b_cidx);
-  d.sp_stageS = (double*)(base + off); off += b_stS;
-  d.sp_stageG = (double*)(base + off); off += b_stG;
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) { cudaGetLastError(); return false; }  // (the host vectors die with this frame)
   d.sp_nchunks = nch;
   return true;
 }
@@ -1786,12 +1746,6 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   for (int i = 0; i < nc; ++i) cam_off[i + 1] += cam_off[i];
   { std::vector<int> pos(cam_off.begin(), cam_off.end()); for (int e = 0; e < no; ++e) cam_perm[pos[scam[e]]++] = e; }
 
-  // ---- layout: one slab = [uploaded blob | working set] ----------------------------------------------------------------
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t b_pose = al((size_t)nc * 7 * 8), b_pts = al((size_t)np * 3 * 8), b_dof = al(nc), b_pf = al(np),
-               b_oc = al((size_t)no * 4), b_op = al((size_t)no * 4), b_uv = al((size_t)no * 16),
-               b_info = d.has_info ? al((size_t)no * 24) : 0, b_po = al((size_t)(np + 1) * 4), b_co = al((size_t)(nc + 1) * 4),
-               b_cp = al((size_t)no * 4), b_cpt = al((size_t)no * 4), b_cuv = al((size_t)no * 16);
   d.s_nnzb = (int)s_col.size();
   std::vector<int> s_upper, s_tidx(s_col.size(), 0);
   for (int blk = 0; blk < (int)s_col.size(); ++blk) {
@@ -1803,18 +1757,6 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   }
   d.s_nupper = (int)s_upper.size();
   tr.stamp("covisibility block-CSR");
-  for (int i = 0; i < nc; ++i) g->pcg_nact += (pb->cam_dof ? (pb->cam_dof[i] & 63) : 63) != 0;
-  for (int i = 0; i < nc && !s_col.empty(); ++i) g->pcg_max_row_blocks = std::max(g->pcg_max_row_blocks, s_rowptr[i + 1] - s_rowptr[i]);
-  std::vector<int> chol_plan3;
-  if (d.s_nnzb > 0) g->chol_ok = ba_chol_plan_host(ctx, nc, s_rowptr.data(), s_col.data(), chol_plan3, &g->chol_blocks, &g->chol_smem);
-  const size_t b_ch = al(chol_plan3.size() * 4 + 4);
-  const size_t b_sr = al((size_t)(nc + 1) * 4), b_sc = al((size_t)s_col.size() * 4 + 4);
-  const bool compact_only = shard_world > 1;  // a shard only ever sees the compact reduced layout: no dense 6N x 6N buffer
-  g->rbuf_doubles = d.s_nnzb > 0 ? (size_t)d.s_nnzb * 36 + 2 * (size_t)d.n6 + 8 : 0;
-  const size_t blob = b_pose + b_pts + b_dof + b_pf + b_oc + b_op + b_uv + b_info + b_po + b_co + b_cp + b_sr + 4 * b_sc + b_cpt + b_cuv + b_ch + 256;
-  const size_t n6 = 6 * (size_t)nc;
-  uint8_t* dblob = nullptr;
-  double* cam_ticket_d = nullptr;
   {  // camera-pass split: ~256 observations per CTA, at most 16 CTAs per camera
     int max_obs = 0;
     for (int i = 0; i < nc; ++i) max_obs = std::max(max_obs, cam_off[i + 1] - cam_off[i]);
@@ -1822,8 +1764,69 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
     // CTA outweighs the shorter serial slices) -> split only cameras that would otherwise run alone for a long time
     d.cam_split = std::min(16, std::max(1, max_obs / 8192));
   }
+
+  // ---- plans: host only, from the host structure above --------------------------------------------------------------------
+  std::vector<uint8_t> dof(nc), pfree(np);
+  for (int i = 0; i < nc; ++i) dof[i] = pb->cam_dof ? (pb->cam_dof[i] & 63) : 63;
+  for (int j = 0; j < np; ++j) pfree[j] = pb->point_free ? (pb->point_free[lo + j] ? 1 : 0) : 1;
+  for (int i = 0; i < nc; ++i) g->pcg_nact += dof[i] != 0;
+  for (int i = 0; i < nc && !s_col.empty(); ++i) g->pcg_max_row_blocks = std::max(g->pcg_max_row_blocks, s_rowptr[i + 1] - s_rowptr[i]);
+  std::vector<int> chol_plan3;
+  if (d.s_nnzb > 0) g->chol_ok = ba_chol_plan_host(ctx, nc, s_rowptr.data(), s_col.data(), chol_plan3, &g->chol_blocks, &g->chol_smem);
+  const bool compact_only = shard_world > 1;  // a shard only ever sees the compact reduced layout: no dense 6N x 6N buffer
+  g->rbuf_doubles = d.s_nnzb > 0 ? (size_t)d.s_nnzb * 36 + 2 * (size_t)d.n6 + 8 : 0;
+  ba_pick_pcg(ctx, g);
+  BaPosePlan pose;
+  if (npe > 0) {  // pose-graph terms: the stepwise path on the dense reduced system (one-cluster / generic PCG)
+    g->pcg_sparse = false;
+    ba_pose_plan(g, pose_edges, pose);
+  }
+  std::vector<int> bcsr_cta_cam;
+  BaSchurPlan schur;
+  if (npe == 0 && (!g->pcg_sparse || compact_only) && d.s_nnzb > 0) {  // (a shard always runs on the compact block-CSR system)
+    ba_pcg_bcsr_plan(ctx, g, s_rowptr.data(), s_col.data(), bcsr_cta_cam);
+    if (!getenv("GB_BA_NO_SCHUR_CHUNKS")) ba_schur_plan(ctx, g, np, pt_off, scam, pfree.data(), s_rowptr, s_col, s_upper, schur);  // (optional: the block-gather kernel otherwise)
+  }
+  if (compact_only && !g->pcg_bcsr) {
+    gb_set_error(ctx, "gb_ba: the sharded solve needs the block-CSR reduced system (<= %d cameras)", kMaxBlockCams);
+    return GB_ERR_INVALID;
+  }
+  std::vector<int> o_pt(no), c_pt(no);
+  for (int e = 0; e < no; ++e) o_pt[e] = pb->obs_point[order[e]] - lo;
+  for (int idx = 0; idx < no; ++idx) c_pt[idx] = o_pt[cam_perm[idx]];
+  tr.stamp("plans");
+
+  // ---- layout: one slab = [uploaded blob | working set] ----------------------------------------------------------------
+  const size_t n6 = 6 * (size_t)nc;
   auto layout = [&](Slab& sl) {
-    sl.take(&dblob, blob);
+    sl.put(&g->pose_wc_in, (size_t)nc * 7, pb->cam_pose_wc);  // T_wc as given: the source of ba_prepare_kernel
+    sl.put(&g->pts_init, (size_t)np * 3, pb->points + 3 * (size_t)lo);
+    sl.put(&d.dof, nc, dof.data()); sl.put(&d.pfree, np, pfree.data());
+    sl.put(&d.o_cam, no, scam.data()); sl.put(&d.o_pt, no, o_pt.data());
+    sl.put(&d.o_uv, 2 * (size_t)no);  // (the measurements: ba_fill_measurements)
+    if (d.has_info) sl.put(&d.o_info, 3 * (size_t)no);
+    sl.put(&d.c_pt, no, c_pt.data()); sl.put(&d.c_uv, 2 * (size_t)no);
+    sl.put(&d.pt_off, pt_off.size(), pt_off.data()); sl.put(&d.cam_off, cam_off.size(), cam_off.data());
+    sl.put(&d.cam_perm, no, cam_perm.data());
+    sl.put(&d.s_rowptr, s_rowptr.size(), s_rowptr.data()); sl.put(&d.s_col, s_col.size(), s_col.data());
+    sl.put(&d.s_brow, s_brow.size(), s_brow.data()); sl.put(&d.s_upper, s_upper.size(), s_upper.data());
+    sl.put(&d.s_tidx, s_tidx.size(), s_tidx.data());
+    sl.put(&g->chol_plan, chol_plan3.size(), chol_plan3.data());
+    if (g->pcg_bcsr) sl.put(&g->bcsr_cta_cam, bcsr_cta_cam.size(), bcsr_cta_cam.data());
+    if (d.sp_nchunks > 0) {
+      sl.put(&d.sp_pt0, schur.pt0.size(), schur.pt0.data()); sl.put(&d.sp_order, schur.order.size(), schur.order.data());
+      sl.put(&d.sp_mask, schur.mask.size(), schur.mask.data()); sl.put(&d.sp_nused, schur.nused.size(), schur.nused.data());
+      sl.put(&d.sp_slots, schur.slots.size(), schur.slots.data());
+      sl.put(&d.sp_boff, schur.boff.size(), schur.boff.data()); sl.put(&d.sp_bidx, schur.bidx.size(), schur.bidx.data());
+      sl.put(&d.sp_coff, schur.coff.size(), schur.coff.data()); sl.put(&d.sp_cidx, schur.cidx.size(), schur.cidx.data());
+    }
+    if (npe > 0) {
+      sl.put(&d.pe_i, pose.ei.size(), pose.ei.data()); sl.put(&d.pe_j, pose.ej.size(), pose.ej.data());
+      sl.put(&d.pe_Zinv, pose.Zinv.size(), pose.Zinv.data()); sl.put(&d.pe_info, pose.info.size(), pose.info.data());
+      sl.put(&d.pc_off, pose.pc_off.size(), pose.pc_off.data()); sl.put(&d.pc_ent, pose.pc_ent.size(), pose.pc_ent.data());
+      sl.put(&d.pp_off, pose.pp_off.size(), pose.pp_off.data()); sl.put(&d.pp_ij, pose.pp_ij.size(), pose.pp_ij.data());
+      sl.put(&d.pp_ent, pose.pp_ent.size(), pose.pp_ent.data());
+    }
     sl.take(&g->pose_init, (size_t)nc * 7); sl.take(&g->pose_wc_out, (size_t)nc * 7);
     sl.take(&d.pose, (size_t)nc * 7); sl.take(&d.pose_new, (size_t)nc * 7);
     sl.take(&d.Rt, (size_t)nc * 12); sl.take(&d.Rt_new, (size_t)nc * 12);
@@ -1831,7 +1834,7 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
     sl.take(&d.V, (size_t)np * 9); sl.take(&d.gp, (size_t)np * 3); sl.take(&d.Vinv, (size_t)np * 9);
     sl.take(&d.W, (size_t)no * 18); sl.take(&d.U, (size_t)nc * 36); sl.take(&d.gc, (size_t)nc * 6);
     sl.take(&d.cost_pt, (size_t)np + npe); sl.take(&d.cost_pt_new, (size_t)np + npe);
-    sl.take(&d.cam_part, (size_t)nc * std::max(d.cam_split, 4) * 27); sl.take(&cam_ticket_d, (size_t)nc / 2 + 1);
+    sl.take(&d.cam_part, (size_t)nc * std::max(d.cam_split, 4) * 27); sl.take(&d.cam_ticket, (size_t)nc + 2);
     sl.take(&d.Minv, (size_t)nc * 36);
     sl.take(&d.Sb, (size_t)d.s_nnzb * 36);
     sl.take(&d.x, n6); sl.take(&d.r, n6); sl.take(&d.z, n6); sl.take(&d.p, n6); sl.take(&d.q, n6); sl.take(&d.sv, n6);
@@ -1840,114 +1843,55 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
     sl.take(&g->buf, compact_only ? 8 : g->buf_doubles);
     sl.take(&g->d_cost, 8);
     sl.take(&g->rbuf, g->rbuf_doubles);
+    if (g->pcg_bcsr) { sl.take(&g->bcsr_part, 2 * (size_t)g->bcsr_ctas); sl.take(&g->bcsr_u, n6); sl.take(&g->bcsr_bar, 16); }
+    if (d.sp_nchunks > 0) {
+      sl.take(&d.sp_stageS, (size_t)d.sp_nchunks * kChunkSlots * 36);
+      sl.take(&d.sp_stageG, (size_t)d.sp_nchunks * kChunkCams * 6);
+    }
+    if (npe > 0) sl.take(&d.pe_H, pose.rec_doubles);
   };
   Slab measure;
   layout(measure);
   const size_t need = measure.off + 256;
-  if (use_arena && !ctx->ba_arena_busy) {
-    if (need > ctx->ba_arena_cap) {
-      GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-      cudaFree(ctx->ba_arena);
-      ctx->ba_arena = nullptr;
-      ctx->ba_arena_cap = 0;
-      const size_t want = need + need / 4;
-      GB_CUDA(ctx, cudaMalloc(&ctx->ba_arena, want));
-      ctx->ba_arena_cap = want;
-    }
+  g->from_arena = use_arena && !ctx->ba_arena_busy;
+  if (g->from_arena && need > ctx->ba_arena_cap) {  // grow the arena (with a quarter to spare: windows grow a little at a time)
+    GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->ba_arena);
+    ctx->ba_arena = nullptr;
+    ctx->ba_arena_cap = 0;
+  }
+  void** dst = g->from_arena ? &ctx->ba_arena : (void**)&g->slab;
+  if (!*dst) {
+    const size_t bytes = g->from_arena ? need + need / 4 : need;
+    GB_CUDA(ctx, cudaMalloc(dst, bytes));
+    if (g->from_arena) ctx->ba_arena_cap = bytes;
+  }
+  if (g->from_arena) {
     g->slab = (uint8_t*)ctx->ba_arena;
-    g->from_arena = true;
     ctx->ba_arena_busy = true;
-  } else {
-    GB_CUDA(ctx, cudaMalloc((void**)&g->slab, need));
   }
   g->slab_bytes = need;
-  Slab real;
-  real.base = g->slab;
-  layout(real);
-
   tr.stamp("slab");
+
   // ---- one pinned blob, one H2D ------------------------------------------------------------------------------------------
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + blob + 4096));
-  uint8_t* h = (uint8_t*)gb_stage_alloc(ctx, blob);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += bytes; return o; };
-  const size_t o_pose = take(b_pose), o_pts = take(b_pts), o_dof = take(b_dof), o_pf = take(b_pf), o_oc = take(b_oc),
-               o_op = take(b_op), o_uv = take(b_uv), o_info = take(b_info), o_po = take(b_po), o_co = take(b_co), o_cp = take(b_cp),
-               o_sr = take(b_sr), o_sc = take(b_sc), o_sb = take(b_sc), o_su = take(b_sc), o_st = take(b_sc), o_cpt = take(b_cpt), o_cuv = take(b_cuv), o_ch = take(b_ch);
-  memcpy(h + o_pose, pb->cam_pose_wc, (size_t)nc * 56);
-  if (np > 0) memcpy(h + o_pts, pb->points + 3 * (size_t)lo, (size_t)np * 24);
-  for (int i = 0; i < nc; ++i) h[o_dof + i] = pb->cam_dof ? (pb->cam_dof[i] & 63) : 63;
-  for (int j = 0; j < np; ++j) h[o_pf + j] = pb->point_free ? (pb->point_free[lo + j] ? 1 : 0) : 1;
-  int* hoc = (int*)(h + o_oc); int* hop = (int*)(h + o_op); double* huv = (double*)(h + o_uv); double* hin = (double*)(h + o_info);
-  for (int e = 0; e < no; ++e) {
-    const int k = order[e];
-    hoc[e] = scam[e];
-    hop[e] = pb->obs_point[k] - lo;
-    const double* m = pb->obs_xyz + 3 * (size_t)k;
-    huv[2 * e] = m[0] / m[2];
-    huv[2 * e + 1] = m[1] / m[2];
-    if (d.has_info) {
-      const double* L = pb->obs_info + 4 * (size_t)k;
-      hin[3 * e] = L[0]; hin[3 * e + 1] = 0.5 * (L[1] + L[2]); hin[3 * e + 2] = L[3];
-    }
-  }
-  memcpy(h + o_po, pt_off.data(), (size_t)(np + 1) * 4);
-  memcpy(h + o_co, cam_off.data(), (size_t)(nc + 1) * 4);
-  memcpy(h + o_cp, cam_perm.data(), (size_t)no * 4);
-  {
-    int* hcpt = (int*)(h + o_cpt);
-    double* hcuv = (double*)(h + o_cuv);
-    for (int idx = 0; idx < no; ++idx) {
-      const int e = cam_perm[idx];
-      hcpt[idx] = hop[e];
-      hcuv[2 * idx] = huv[2 * e];
-      hcuv[2 * idx + 1] = huv[2 * e + 1];
-    }
-  }
-  memcpy(h + o_sr, s_rowptr.data(), (size_t)(nc + 1) * 4);
-  if (!s_col.empty()) memcpy(h + o_sc, s_col.data(), s_col.size() * 4);
-  if (!s_brow.empty()) memcpy(h + o_sb, s_brow.data(), s_brow.size() * 4);
-  if (!s_upper.empty()) memcpy(h + o_su, s_upper.data(), s_upper.size() * 4);
-  if (!s_tidx.empty()) memcpy(h + o_st, s_tidx.data(), s_tidx.size() * 4);
-  if (!chol_plan3.empty()) memcpy(h + o_ch, chol_plan3.data(), chol_plan3.size() * 4);
-  g->chol_plan = (const int*)(dblob + o_ch);
+  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + measure.blob + 4096));
+  Slab real{g->slab, (uint8_t*)gb_stage_alloc(ctx, measure.blob)};
+  layout(real);
+  ba_fill_measurements(pb, order, cam_perm, real.host(d.o_uv), real.host(d.c_uv), d.has_info ? real.host(d.o_info) : nullptr);
   g->sorted_to_orig.swap(order);
   g->cam_perm_h.swap(cam_perm);
   g->pt_off_h = pt_off; g->cam_off_h = cam_off;  // (the large-graph sweep cuts its work items from these on first use)
   tr.stamp("blob fill");
-  GB_CUDA(ctx, cudaMemcpyAsync(dblob, h, blob, cudaMemcpyHostToDevice, ctx->stream));
-  d.cam_ticket = reinterpret_cast<unsigned int*>(cam_ticket_d);
+  GB_CUDA(ctx, cudaMemcpyAsync(real.base, real.h, real.blob, cudaMemcpyHostToDevice, ctx->stream));
   d.red_ticket = reinterpret_cast<unsigned int*>(d.red_part + kRedPartials);
   GB_CUDA(ctx, cudaMemsetAsync(d.red_ticket, 0, 16, ctx->stream));
-  GB_CUDA(ctx, cudaMemsetAsync(d.cam_ticket, 0, ((size_t)nc / 2 + 1) * 8, ctx->stream));
-  double* d_pose_wc = (double*)(dblob + o_pose);
-  g->pose_wc_in = d_pose_wc;
-  g->pts_init = (double*)(dblob + o_pts);
-  d.dof = dblob + o_dof; d.pfree = dblob + o_pf;
-  d.o_cam = (int*)(dblob + o_oc); d.o_pt = (int*)(dblob + o_op); d.o_uv = (double*)(dblob + o_uv);
-  d.o_info = d.has_info ? (double*)(dblob + o_info) : nullptr;
-  d.pt_off = (int*)(dblob + o_po); d.cam_off = (int*)(dblob + o_co); d.cam_perm = (int*)(dblob + o_cp);
-  d.c_pt = (int*)(dblob + o_cpt); d.c_uv = (double*)(dblob + o_cuv);
-  d.s_rowptr = (int*)(dblob + o_sr); d.s_col = (int*)(dblob + o_sc); d.s_brow = (int*)(dblob + o_sb);
-  d.s_upper = (int*)(dblob + o_su); d.s_tidx = (int*)(dblob + o_st);
+  GB_CUDA(ctx, cudaMemsetAsync(d.cam_ticket, 0, ((size_t)nc + 2) * 4, ctx->stream));
+  if (npe > 0) GB_CUDA(ctx, cudaMemsetAsync(d.pe_H, 0, pose.rec_doubles * 8, ctx->stream));
   if (nc > 0) {
-    ba_prepare_kernel<<<gb_div_up(nc, 128), 128, 0, ctx->stream>>>(nc, d_pose_wc, g->pose_init);
+    ba_prepare_kernel<<<gb_div_up(nc, 128), 128, 0, ctx->stream>>>(nc, g->pose_wc_in, g->pose_init);
     GB_LAUNCH_CHECK(ctx);
   }
   GB_CHECK(gb_ba_graph_reset(ctx, g));
-  ba_pick_pcg(ctx, g);
-  if (npe > 0) {  // pose-graph terms: the stepwise path on the dense reduced system (one-cluster / generic PCG)
-    g->pcg_sparse = false;
-    GB_CHECK(ba_pose_attach(ctx, g, pose_edges));
-  }
-  if (npe == 0 && (!g->pcg_sparse || compact_only) && d.s_nnzb > 0) {  // (a shard always runs on the compact block-CSR system)
-    GB_CHECK(ba_pcg_bcsr_plan(ctx, g, s_rowptr.data(), s_col.data()));
-    if (!getenv("GB_BA_NO_SCHUR_CHUNKS")) ba_schur_plan(ctx, g, np, pt_off, scam, h + o_pf, s_rowptr, s_col, s_upper);  // (optional: the block-gather kernel otherwise)
-  }
-  if (compact_only && !g->pcg_bcsr) {
-    gb_set_error(ctx, "gb_ba: the sharded solve needs the block-CSR reduced system (<= %d cameras)", kMaxBlockCams);
-    return GB_ERR_INVALID;
-  }
   tr.stamp("enqueue H2D + prepare");
   // the pinned blob is reused by the next outermost call on this ctx: a graph handed to the caller must have consumed it; the
   // one-shot host-buffer paths (gb_ba_solve / gb_ba_pnp) synchronise in their own finish + download before they return
@@ -2025,13 +1969,8 @@ static int ba_pcg_generic(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
 
 // local-BA PCG: one thread-block cluster, S resident in shared memory, one cluster barrier per iteration
 static int ba_pcg_cluster(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(g->pcg_cluster); cfg.blockDim = dim3(kPcgThreads); cfg.dynamicSmemBytes = g->pcg_smem; cfg.stream = ctx->stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = g->pcg_cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  GB_CUDA(ctx, cudaLaunchKernelEx(&cfg, ba_pcg_cluster_kernel, g->d, buf, (int)g->opt.pcg_max_iters));
+  GbClusterConfig lc(g->pcg_cluster, dim3(kPcgThreads), g->pcg_smem, ctx->stream);
+  GB_CUDA(ctx, cudaLaunchKernelEx(&lc.cfg, ba_pcg_cluster_kernel, g->d, buf, (int)g->opt.pcg_max_iters));
   GB_LAUNCH_CHECK(ctx);
   return GB_OK;
 }
@@ -2347,10 +2286,7 @@ void ba_cache_drop(gb_ctx* ctx) {
 static int ba_graph_refresh(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_problem* pb) {
   BaDev& d = g->d;
   const int nc = d.nc, np = d.np, no = d.no;
-  for (int k = 0; k < no; ++k) {
-    const double z = pb->obs_xyz[3 * (size_t)k + 2];
-    if (!(z != 0.0) || !std::isfinite(z)) { gb_set_error(ctx, "gb_ba: edge %d has a zero/non-finite measurement z", k); return GB_ERR_INVALID; }
-  }
+  for (int k = 0; k < no; ++k) GB_CHECK(ba_check_z(ctx, pb, k));
   const size_t b_pose = (size_t)nc * 56, b_pts = (size_t)np * 24, b_uv = (size_t)no * 16, b_info = d.has_info ? (size_t)no * 24 : 0;
   GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + b_pose + b_pts + 2 * b_uv + b_info + 4096));
   double* h_pose = (double*)gb_stage_alloc(ctx, b_pose + 8);
@@ -2361,21 +2297,7 @@ static int ba_graph_refresh(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_problem* pb
   if (!h_pose || !h_pts || !h_uv || !h_cuv || (b_info && !h_info)) { gb_set_error(ctx, "gb_ba: staging exhausted"); return GB_ERR_CUDA; }
   memcpy(h_pose, pb->cam_pose_wc, b_pose);
   memcpy(h_pts, pb->points, b_pts);
-  for (int e = 0; e < no; ++e) {
-    const int k = g->sorted_to_orig[e];
-    const double* m = pb->obs_xyz + 3 * (size_t)k;
-    h_uv[2 * e] = m[0] / m[2];
-    h_uv[2 * e + 1] = m[1] / m[2];
-    if (h_info) {
-      const double* L = pb->obs_info + 4 * (size_t)k;
-      h_info[3 * e] = L[0]; h_info[3 * e + 1] = 0.5 * (L[1] + L[2]); h_info[3 * e + 2] = L[3];
-    }
-  }
-  for (int idx = 0; idx < no; ++idx) {
-    const int e = g->cam_perm_h[idx];
-    h_cuv[2 * idx] = h_uv[2 * e];
-    h_cuv[2 * idx + 1] = h_uv[2 * e + 1];
-  }
+  ba_fill_measurements(pb, g->sorted_to_orig, g->cam_perm_h, h_uv, h_cuv, h_info);
   cudaStream_t s = ctx->stream;
   if (nc > 0) GB_CUDA(ctx, cudaMemcpyAsync(g->pose_wc_in, h_pose, b_pose, cudaMemcpyHostToDevice, s));
   if (np > 0) GB_CUDA(ctx, cudaMemcpyAsync(g->pts_init, h_pts, b_pts, cudaMemcpyHostToDevice, s));

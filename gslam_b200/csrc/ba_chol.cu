@@ -230,20 +230,7 @@ bool ba_chol_plan_host(gb_ctx* ctx, int nc, const int* s_rowptr, const int* s_co
   }
   const size_t smem = ((size_t)nb * 36 + 12 * (size_t)nc) * sizeof(double) + 3 * (size_t)nc * sizeof(int) + 64;
   if (smem + 1024 > (size_t)ctx->max_smem_optin) return false;
-  {
-    static std::mutex mu;
-    static int state[64] = {0};
-    std::lock_guard<std::mutex> lk(mu);
-    const int dev = ctx->device;
-    if (dev < 0 || dev >= 64) return false;
-    if (state[dev] == 0) {
-      cudaFuncAttributes fa;
-      state[dev] = (cudaFuncGetAttributes(&fa, ba_chol_kernel) == cudaSuccess &&
-                    cudaFuncSetAttribute(ba_chol_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->max_smem_optin - (int)fa.sharedSizeBytes) == cudaSuccess) ? 1 : 2;
-      cudaGetLastError();
-    }
-    if (state[dev] != 1) return false;
-  }
+  if (!gb_func_setup(ctx, (const void*)ba_chol_kernel, GB_SMEM_OPTIN_MAX)) return false;
   *nblocks = (int)nb; *smem_out = smem;
   return true;
 }

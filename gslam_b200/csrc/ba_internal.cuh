@@ -2,14 +2,51 @@
 // (ba.cu: graph upload, kernels of the sweep / Schur / local PCG paths; ba_pcg_bcsr.cu: the multi-CTA block-CSR PCG of large
 // reduced systems; ba_dist.cu: the landmark-sharded multi-GPU solve and its communicator).  Not part of the C-ABI.
 #pragma once
+#include <type_traits>
 #include <vector>
 
 #include "ba_device.cuh"
 #include "common.cuh"
 
+// Layout of one device allocation, written as ONE list of declarations that is run twice: first to measure (base == nullptr),
+// then to place the arrays at base.  put() declares an uploaded array and copies its host source, if it has one, into the pinned
+// staging h at the array's offset; the puts come first, so [0, blob) is one contiguous upload.  take() declares device-only
+// working memory after them.  Every array starts on a 256-byte boundary (kernels such as cta_copy_f64 rely on it).
+struct Slab {
+  uint8_t* base = nullptr;
+  uint8_t* h = nullptr;  // host staging mirror of [0, blob)
+  size_t off = 0, blob = 0;
+  template <typename T>
+  void take(T** p, size_t n) {
+    off = (off + 255) & ~(size_t)255;
+    if (base) *p = (T*)(base + off);
+    off += std::max<size_t>(n, 1) * sizeof(T);
+  }
+  template <typename T>
+  void put(T** p, size_t n, const std::remove_const_t<T>* src = nullptr) {
+    take(p, n);
+    blob = off;
+    if (h && src && n) memcpy(h + ((const uint8_t*)*p - base), src, n * sizeof(T));
+  }
+  template <typename T>
+  std::remove_const_t<T>* host(T* p) const { return (std::remove_const_t<T>*)(h + ((const uint8_t*)p - base)); }  // staging of a put array
+};
+
+// host-made plans of graph creation, uploaded with the graph (ba_graph_create_impl lays them out)
+struct BaSchurPlan {  // landmark-chunk Schur complement: BaDev::sp_*
+  std::vector<int> pt0, order, nused, boff, bidx, coff, cidx;
+  std::vector<unsigned short> mask;
+  std::vector<uint8_t> slots;
+};
+struct BaPosePlan {  // pose-graph edges and their gather plans: BaDev::pe_* / pc_* / pp_*
+  std::vector<int> ei, ej, pc_off, pc_ent, pp_off, pp_ij, pp_ent;
+  std::vector<double> Zinv, info;
+  size_t rec_doubles = 0;  // pe_H: staging records of every edge (zeroed at creation)
+};
+
 struct gb_ba_graph {
   BaDev d{};
-  uint8_t* slab = nullptr;  // one device allocation (or the ctx arena) holding everything below
+  uint8_t* slab = nullptr;  // one device allocation (or the ctx arena) holding everything below but the sweep plan
   size_t slab_bytes = 0;
   bool from_arena = false;
   double *pose_init = nullptr, *pts_init = nullptr, *pose_wc_out = nullptr;
@@ -36,7 +73,7 @@ struct gb_ba_graph {
   int bcsr_ctas = 0, bcsr_K = 0, bcsr_in_smem = 0, bcsr_max_cams = 0, bcsr_max_blocks = 0, bcsr_cluster = 0, bcsr_blk_stride = 37;
   size_t bcsr_smem = 0;
   unsigned short bcsr_need[16] = {0};  // cluster mode: bcsr_need[c] = CTAs that read the rows of u owned by CTA c
-  int* bcsr_cta_cam = nullptr;   // device [bcsr_ctas + 1]: first camera of each CTA's block-row range (base of one allocation)
+  const int* bcsr_cta_cam = nullptr;  // device [bcsr_ctas + 1]: first camera of each CTA's block-row range
   double* bcsr_part = nullptr;   // device [bcsr_ctas * 2]: per-CTA (gamma, delta) partials
   double* bcsr_u = nullptr;      // device [n6]: the published u = Minv r
   unsigned int* bcsr_bar = nullptr;  // device: grid barrier counter
@@ -47,8 +84,6 @@ struct gb_ba_graph {
   const int* chol_plan = nullptr;
   int chol_blocks = 0;
   size_t chol_smem = 0;
-  void* sp_alloc = nullptr;      // device allocation holding the landmark-chunk Schur plan + staging (BaDev::sp_*), or null
-  void* pe_alloc = nullptr;      // device allocation holding the pose-graph edges and their gather plans (BaDev::pe_* / pc_* / pp_*)
   void* sw_alloc = nullptr;      // device allocation holding the large-graph sweep's item plan (BaDev::sw_*), made on first use
   std::vector<int> pt_off_h, cam_off_h;  // host copies of pt_off / cam_off (the sweep plan is cut from them)
   // landmark shard (multi-GPU global BA): this graph holds landmarks [shard_lo, shard_hi) of the caller's problem
@@ -68,8 +103,7 @@ int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
 // ---- ba_pose.cu -------------------------------------------------------------------------------------------------------------
 // pose-graph terms (SE3Edge / GPSEdge, Optimizer.h:127-148) on the stepwise dense-layout solver path
 int ba_pose_validate(gb_ctx* ctx, const gb_ba_problem* pb, const gb_pose_edges* pe);
-int ba_pose_attach(gb_ctx* ctx, gb_ba_graph* g, const gb_pose_edges* pe);   // upload edges + gather plans (graph creation)
-void ba_pose_free(gb_ba_graph* g);
+void ba_pose_plan(gb_ba_graph* g, const gb_pose_edges* pe, BaPosePlan& p);  // host-only: edges + gather plans, sets d.npe / d.pe_npairs
 int ba_pose_linearize(gb_ctx* ctx, gb_ba_graph* g, cudaStream_t s);         // after the sweep: records -> U, g_c, cost terms
 int ba_pose_offdiag(gb_ctx* ctx, gb_ba_graph* g, double* buf, cudaStream_t s);  // after the Schur complement: S_ij += J_i' Omega J_j
 int ba_pose_cost(gb_ctx* ctx, gb_ba_graph* g, cudaStream_t s);              // candidate cost terms at pose_new
@@ -82,9 +116,9 @@ void ba_sweep_plan_drop(gb_ba_graph* g);  // (cam_split changed / graph destroye
 int ba_sweep_launch(gb_ctx* ctx, gb_ba_graph* g, const BaDev& d, cudaStream_t s, int which /* 3 whole, 1 cameras, 2 landmarks */);
 
 // ---- ba_pcg_bcsr.cu ---------------------------------------------------------------------------------------------------------
-// Decide whether / how the multi-CTA block-CSR PCG applies to `g` (fills the bcsr_* fields, allocates its small device buffers).
-int ba_pcg_bcsr_plan(gb_ctx* ctx, gb_ba_graph* g, const int* s_rowptr_host, const int* s_col_host);
-void ba_pcg_bcsr_free(gb_ba_graph* g);
+// Host-only: decide whether / how the multi-CTA block-CSR PCG applies to `g` (sets pcg_bcsr and the scalar bcsr_* fields, fills
+// cta_cam, the first camera of each CTA's block-row range).
+void ba_pcg_bcsr_plan(gb_ctx* ctx, gb_ba_graph* g, const int* s_rowptr_host, const int* s_col_host, std::vector<int>& cta_cam);
 // damp + block-Jacobi PCG on the reduced camera system held in `rbuf` + retraction of the cameras (pose_new, Rt_new, x)
 int ba_pcg_bcsr_launch(gb_ctx* ctx, gb_ba_graph* g, const double* rbuf);
 

@@ -328,32 +328,15 @@ static void bcsr_partition(int nc, int nnzb, const int* s_rowptr, int G, std::ve
   }
 }
 
-int ba_pcg_bcsr_plan(gb_ctx* ctx, gb_ba_graph* g, const int* s_rowptr, const int* s_col_host) {
+void ba_pcg_bcsr_plan(gb_ctx* ctx, gb_ba_graph* g, const int* s_rowptr, const int* s_col_host, std::vector<int>& cta_cam) {
   g->pcg_bcsr = false;
   const int nc = g->d.nc, nnzb = g->d.s_nnzb, n6 = g->d.n6;
-  if (nc <= 0 || nnzb <= 0) return GB_OK;
-  static bool cluster16_ok[64] = {false};
-  {  // function attributes are per-device state: set them once per device, never lower them
-    static std::mutex mu;
-    static int state[64] = {0};
-    std::lock_guard<std::mutex> lk(mu);
-    const int dev = ctx->device;
-    if (dev < 0 || dev >= 64) return GB_OK;
-    if (state[dev] == 0) {
-      auto raise = [&](const void* fn) {  // (the opt-in maximum covers static + dynamic shared memory)
-        cudaFuncAttributes fa;
-        return cudaFuncGetAttributes(&fa, fn) == cudaSuccess &&
-               cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->max_smem_optin - (int)fa.sharedSizeBytes) == cudaSuccess;
-      };
-      const bool ok = raise((const void*)ba_pcg_bcsr_kernel<false>) && raise((const void*)ba_pcg_bcsr_kernel<true>);
-      cluster16_ok[dev] = cudaFuncSetAttribute(ba_pcg_bcsr_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
-      state[dev] = ok ? 1 : 2;
-      cudaGetLastError();
-    }
-    if (state[dev] != 1) return GB_OK;
-  }
+  if (nc <= 0 || nnzb <= 0) return;
+  bool cluster16_ok = false;
+  if (!gb_func_setup(ctx, (const void*)ba_pcg_bcsr_kernel<false>, GB_SMEM_OPTIN_MAX) ||
+      !gb_func_setup(ctx, (const void*)ba_pcg_bcsr_kernel<true>, GB_SMEM_OPTIN_MAX, &cluster16_ok))
+    return;
   const size_t budget = (size_t)ctx->max_smem_optin - 2048;  // (static shared memory of the kernel: < 1 KB)
-  std::vector<int> cta_cam;
   int G = 0, max_cams = 1, max_blocks = 1, cluster = 0, blk_stride = kBlkStride;
   bool in_smem = true;
   size_t smem = 0;
@@ -362,21 +345,16 @@ int ba_pcg_bcsr_plan(gb_ctx* ctx, gb_ba_graph* g, const int* s_rowptr, const int
     const int sizes[2] = {16, 8};
     for (int t = 0; t < 2 && !cluster; ++t) {
       const int C = std::min(sizes[t], nc);
-      if (C > 8 && !cluster16_ok[ctx->device]) continue;
+      if (C > 8 && !cluster16_ok) continue;
       int mc, mb;
       bcsr_partition(nc, nnzb, s_rowptr, C, cta_cam, &mc, &mb);
       const int strides[2] = {kBlkStride, 36};  // (36: 2-way bank conflicts on the block loads, but 6 % less shared memory)
       for (int q = 0; q < 2 && !cluster; ++q) {
         const size_t need = bcsr_smem_bytes(n6, mc, mb, true, strides[q]);
         if (need > budget) continue;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(C); cfg.blockDim = dim3(kBcsrThreads); cfg.dynamicSmemBytes = need; cfg.stream = ctx->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
+        GbClusterConfig lc(C, dim3(kBcsrThreads), need, ctx->stream);
         int nclusters = 0;
-        if (cudaOccupancyMaxActiveClusters(&nclusters, ba_pcg_bcsr_kernel<true>, &cfg) != cudaSuccess || nclusters < 1) { cudaGetLastError(); continue; }
+        if (cudaOccupancyMaxActiveClusters(&nclusters, ba_pcg_bcsr_kernel<true>, &lc.cfg) != cudaSuccess || nclusters < 1) { cudaGetLastError(); continue; }
         cluster = C; G = C; max_cams = mc; max_blocks = mb; blk_stride = strides[q]; smem = need;
       }
     }
@@ -385,35 +363,24 @@ int ba_pcg_bcsr_plan(gb_ctx* ctx, gb_ba_graph* g, const int* s_rowptr, const int
   if (!cluster) {
     int coop = 0;
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx->device);
-    if (!coop) return GB_OK;
+    if (!coop) return;
     G = std::max(1, std::min(ctx->sm_count, nc));
     bcsr_partition(nc, nnzb, s_rowptr, G, cta_cam, &max_cams, &max_blocks);
     smem = bcsr_smem_bytes(n6, max_cams, max_blocks, true);
     if (smem > budget) {
       in_smem = false;
       smem = bcsr_smem_bytes(n6, max_cams, max_blocks, false);
-      if (smem > budget) return GB_OK;  // not even the vectors fit: generic path
+      if (smem > budget) return;  // not even the vectors fit: generic path
     }
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_pcg_bcsr_kernel<false>, kBcsrThreads, smem) != cudaSuccess || per_sm < 1) {
       cudaGetLastError();
-      return GB_OK;
+      return;
     }
-    if ((long long)per_sm * ctx->sm_count < G) return GB_OK;
+    if ((long long)per_sm * ctx->sm_count < G) return;
   }
   int K = 32;  // lanes per camera in the mat-vec (>= 8: lanes 0..5 publish the six rows)
   while (K > 8 && max_cams * K > kBcsrThreads) K >>= 1;
-  const size_t bytes = (size_t)(G + 1) * 4 + 256 + (size_t)2 * G * 8 + 256 + (size_t)n6 * 8 + 256 + 256;
-  uint8_t* base = nullptr;
-  GB_CUDA(ctx, cudaMalloc((void**)&base, bytes));
-  size_t off = 0;
-  auto take = [&](size_t n) { uint8_t* p = base + off; off = (off + n + 255) & ~(size_t)255; return p; };
-  g->bcsr_cta_cam = (int*)take((size_t)(G + 1) * 4);
-  g->bcsr_part = (double*)take((size_t)2 * G * 8);
-  g->bcsr_u = (double*)take((size_t)n6 * 8);
-  g->bcsr_bar = (unsigned int*)take(64);
-  GB_CUDA(ctx, cudaMemcpyAsync(g->bcsr_cta_cam, cta_cam.data(), (size_t)(G + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // (cta_cam is a stack-lifetime host vector)
   g->bcsr_ctas = G; g->bcsr_K = K; g->bcsr_in_smem = in_smem ? 1 : 0; g->bcsr_smem = smem;
   g->bcsr_max_cams = max_cams; g->bcsr_max_blocks = max_blocks; g->bcsr_cluster = cluster; g->bcsr_blk_stride = blk_stride;
   // who reads whose rows of u (cluster mode: the publication of u only goes where it is needed)
@@ -428,13 +395,6 @@ int ba_pcg_bcsr_plan(gb_ctx* ctx, gb_ba_graph* g, const int* s_rowptr, const int
     }
   }
   g->pcg_bcsr = true;
-  return GB_OK;
-}
-
-void ba_pcg_bcsr_free(gb_ba_graph* g) {
-  if (g->bcsr_cta_cam) cudaFree(g->bcsr_cta_cam);  // (one allocation: cta_cam is its base)
-  g->bcsr_cta_cam = nullptr; g->bcsr_part = nullptr; g->bcsr_u = nullptr; g->bcsr_bar = nullptr;
-  g->pcg_bcsr = false;
 }
 
 int ba_pcg_bcsr_launch(gb_ctx* ctx, gb_ba_graph* g, const double* rbuf) {
@@ -449,13 +409,8 @@ int ba_pcg_bcsr_launch(gb_ctx* ctx, gb_ba_graph* g, const double* rbuf) {
   for (int c = 0; c < 16; ++c) a.need[c] = g->bcsr_need[c];
   double* rb = const_cast<double*>(rbuf);  // (the damped diagonal is written back when S stays in global memory)
   if (g->bcsr_cluster > 0) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(g->bcsr_cluster); cfg.blockDim = dim3(kBcsrThreads); cfg.dynamicSmemBytes = g->bcsr_smem; cfg.stream = ctx->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = g->bcsr_cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    GB_CUDA(ctx, cudaLaunchKernelEx(&cfg, ba_pcg_bcsr_kernel<true>, d, rb, a));
+    GbClusterConfig lc(g->bcsr_cluster, dim3(kBcsrThreads), g->bcsr_smem, ctx->stream);
+    GB_CUDA(ctx, cudaLaunchKernelEx(&lc.cfg, ba_pcg_bcsr_kernel<true>, d, rb, a));
   } else {
     GB_CUDA(ctx, cudaMemsetAsync(g->bcsr_bar, 0, 4, ctx->stream));
     void* args[3] = {(void*)&d, (void*)&rb, (void*)&a};

@@ -246,18 +246,13 @@ int ba_pose_validate(gb_ctx* ctx, const gb_ba_problem* pb, const gb_pose_edges* 
   return GB_OK;
 }
 
-void ba_pose_free(gb_ba_graph* g) {
-  if (g->pe_alloc) cudaFree(g->pe_alloc);
-  g->pe_alloc = nullptr;
-  g->d.npe = 0;
-}
-
-// upload the edges and the two gather plans (camera -> incident records, unordered pair -> records); called from graph creation
-int ba_pose_attach(gb_ctx* ctx, gb_ba_graph* g, const gb_pose_edges* pe) {
+// the edges and the two gather plans (camera -> incident records, unordered pair -> records); graph creation uploads them
+void ba_pose_plan(gb_ba_graph* g, const gb_pose_edges* pe, BaPosePlan& p) {
   BaDev& d = g->d;
   const int nse = pe->n_se3, ngps = pe->n_gps, npe = nse + ngps, nc = d.nc;
-  std::vector<int> ei(npe), ej(npe);
-  std::vector<double> Zinv((size_t)npe * 7), info((size_t)npe * 36);
+  std::vector<int> &ei = p.ei, &ej = p.ej;
+  std::vector<double> &Zinv = p.Zinv, &info = p.info;
+  ei.resize(npe); ej.resize(npe); Zinv.resize((size_t)npe * 7); info.resize((size_t)npe * 36);
   auto inv7 = [](const double* in, double* out) {  // SE3.h:100-103 (as ba_device.cuh::se3_inverse, on the host)
     const double n = std::sqrt(in[0] * in[0] + in[1] * in[1] + in[2] * in[2] + in[3] * in[3]);
     const double q[4] = {-in[0] / n, -in[1] / n, -in[2] / n, in[3] / n};
@@ -278,7 +273,8 @@ int ba_pose_attach(gb_ctx* ctx, gb_ba_graph* g, const gb_pose_edges* pe) {
       for (int b = 0; b < 6; ++b) info[36 * (size_t)k + a * 6 + b] = src ? 0.5 * (src[a * 6 + b] + src[b * 6 + a]) : (a == b ? 1.0 : 0.0);
   }
   // camera -> incident (edge, side) in edge order
-  std::vector<int> pc_off(nc + 1, 0), pc_ent;
+  std::vector<int> &pc_off = p.pc_off, &pc_ent = p.pc_ent;
+  pc_off.assign(nc + 1, 0);
   for (int k = 0; k < npe; ++k) { pc_off[ei[k] + 1]++; if (ej[k] >= 0) pc_off[ej[k] + 1]++; }
   for (int i = 0; i < nc; ++i) pc_off[i + 1] += pc_off[i];
   pc_ent.resize(pc_off[nc]);
@@ -289,7 +285,8 @@ int ba_pose_attach(gb_ctx* ctx, gb_ba_graph* g, const gb_pose_edges* pe) {
   std::iota(order.begin(), order.end(), 0);
   auto key = [&](int k) { return std::make_pair(std::min(ei[k], ej[k]), std::max(ei[k], ej[k])); };
   std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return key(a) < key(b); });
-  std::vector<int> pp_off(1, 0), pp_ij, pp_ent;
+  std::vector<int> &pp_off = p.pp_off, &pp_ij = p.pp_ij, &pp_ent = p.pp_ent;
+  pp_off.assign(1, 0);
   for (int n = 0; n < nse; ++n) {
     const int k = order[n];
     if (n == 0 || key(k) != key(order[n - 1])) {
@@ -299,37 +296,8 @@ int ba_pose_attach(gb_ctx* ctx, gb_ba_graph* g, const gb_pose_edges* pe) {
     pp_ent.push_back(2 * k + (ei[k] > ej[k] ? 1 : 0));
   }
   pp_off.push_back((int)pp_ent.size());
-  const int npairs = (int)pp_ij.size() / 2;
-  // one allocation
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t b_i = al((size_t)npe * 4), b_Z = al((size_t)npe * 56), b_info = al((size_t)npe * 288), b_H = al((size_t)npe * kRec * 8),
-               b_pco = al((size_t)(nc + 1) * 4), b_pce = al(pc_ent.size() * 4 + 4), b_ppo = al(pp_off.size() * 4), b_ppij = al(pp_ij.size() * 4 + 4),
-               b_ppe = al(pp_ent.size() * 4 + 4);
-  const size_t total = 2 * b_i + b_Z + b_info + b_H + b_pco + b_pce + b_ppo + b_ppij + b_ppe;
-  GB_CUDA(ctx, cudaMalloc(&g->pe_alloc, total));
-  uint8_t* base = (uint8_t*)g->pe_alloc;
-  size_t off = 0;
-  auto put = [&](const void* src, size_t bytes, size_t reserve) -> void* {
-    void* dst = base + off;
-    if (bytes) cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
-    off += reserve;
-    return dst;
-  };
-  d.pe_i = (const int*)put(ei.data(), (size_t)npe * 4, b_i);
-  d.pe_j = (const int*)put(ej.data(), (size_t)npe * 4, b_i);
-  d.pe_Zinv = (const double*)put(Zinv.data(), (size_t)npe * 56, b_Z);
-  d.pe_info = (const double*)put(info.data(), (size_t)npe * 288, b_info);
-  d.pe_H = (double*)put(nullptr, 0, b_H);
-  d.pc_off = (const int*)put(pc_off.data(), (size_t)(nc + 1) * 4, b_pco);
-  d.pc_ent = (const int*)put(pc_ent.data(), pc_ent.size() * 4, b_pce);
-  d.pp_off = (const int*)put(pp_off.data(), pp_off.size() * 4, b_ppo);
-  d.pp_ij = (const int*)put(pp_ij.data(), pp_ij.size() * 4, b_ppij);
-  d.pp_ent = (const int*)put(pp_ent.data(), pp_ent.size() * 4, b_ppe);
-  GB_CUDA(ctx, cudaMemsetAsync(d.pe_H, 0, b_H, ctx->stream));
-  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // (the host vectors die with this frame)
-  GB_CUDA(ctx, cudaGetLastError());
-  d.npe = npe; d.pe_npairs = npairs;
-  return GB_OK;
+  p.rec_doubles = (size_t)npe * kRec;
+  d.npe = npe; d.pe_npairs = (int)pp_ij.size() / 2;
 }
 
 // after the sweep: edge records, then their sums into U / g_c

@@ -441,17 +441,6 @@ static size_t ba_sweep_smem(int nc) {
   return (size_t)kOffPose * sizeof(double) + (pose ? (size_t)nc * kPoseStride * 8 + (((size_t)nc + 15) & ~(size_t)15) : 0);
 }
 
-static int ba_sweep_setup(gb_ctx* ctx) {  // once per device: opt in to the large dynamic shared memory (never lowered)
-  static std::once_flag once[64];
-  cudaError_t e = cudaSuccess;
-  std::call_once(once[ctx->device & 63], [&] {
-    e = cudaFuncSetAttribute(ba_sweep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ba_sweep_smem(kSwPoseCams));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ba_sweep_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ba_sweep_smem(kSwPoseCams + 1));
-  });
-  if (e != cudaSuccess) { gb_set_error(ctx, "ba_sweep_setup: %s", cudaGetErrorString(e)); return GB_ERR_CUDA; }
-  return GB_OK;
-}
-
 void ba_sweep_plan_drop(gb_ba_graph* g) {
   if (g->sw_alloc) cudaFree(g->sw_alloc);
   g->sw_alloc = nullptr;
@@ -463,19 +452,35 @@ static int ba_sweep_plan(gb_ctx* ctx, gb_ba_graph* g) {
   std::vector<int> items4, team_off;
   const int n_teams = ba_sweep_teams(ctx);
   ba_sweep_plan_host(g->d.nc, g->d.np, g->d.cam_split, g->cam_off_h, g->pt_off_h, n_teams, items4, team_off);
-  const size_t b_items = (items4.size() * 4 + 255) & ~(size_t)255, b_off = team_off.size() * 4;
-  GB_CUDA(ctx, cudaMalloc(&g->sw_alloc, b_items + b_off + 256));
-  uint8_t* base = (uint8_t*)g->sw_alloc;
-  if (!items4.empty()) GB_CUDA(ctx, cudaMemcpyAsync(base, items4.data(), items4.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-  GB_CUDA(ctx, cudaMemcpyAsync(base + b_items, team_off.data(), b_off, cudaMemcpyHostToDevice, ctx->stream));
-  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // (the host vectors die with this frame)
-  g->d.sw_items = (const int*)base; g->d.sw_team_off = (const int*)(base + b_items);
+  auto layout = [&](Slab& sl) {
+    sl.put(&g->d.sw_items, items4.size(), items4.data());
+    sl.put(&g->d.sw_team_off, team_off.size(), team_off.data());
+  };
+  Slab measure;
+  layout(measure);
+  // (pageable staging: this runs in the middle of an API call, where the ctx's pinned staging must not be reserved)
+  std::vector<uint8_t> h(measure.blob);
+  GB_CUDA(ctx, cudaMalloc(&g->sw_alloc, measure.off));
+  Slab real{(uint8_t*)g->sw_alloc, h.data()};
+  layout(real);
+  cudaError_t e = cudaMemcpyAsync(real.base, real.h, real.blob, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);  // (h dies with this frame)
+  if (e != cudaSuccess) {
+    ba_sweep_plan_drop(g);  // (no half-made plan: the next launch plans again)
+    gb_set_error(ctx, "ba_sweep: plan upload -> %s", cudaGetErrorString(e));
+    return GB_ERR_CUDA;
+  }
   g->d.sw_nteams = n_teams; g->d.sw_nitems = (int)(items4.size() / 4);
   return GB_OK;
 }
 
 int ba_sweep_launch(gb_ctx* ctx, gb_ba_graph* g, const BaDev& d_in, cudaStream_t s, int which) {
-  GB_CHECK(ba_sweep_setup(ctx));
+  // once per device: opt in to the large dynamic shared memory
+  if (!gb_func_setup(ctx, (const void*)ba_sweep_kernel<true>, (int)ba_sweep_smem(kSwPoseCams)) ||
+      !gb_func_setup(ctx, (const void*)ba_sweep_kernel<false>, (int)ba_sweep_smem(kSwPoseCams + 1))) {
+    gb_set_error(ctx, "ba_sweep: cannot set the shared-memory limit of the sweep kernel");
+    return GB_ERR_CUDA;
+  }
   if (!g->sw_alloc) GB_CHECK(ba_sweep_plan(ctx, g));
   if (g->d.sw_nitems <= 0) return GB_OK;
   BaDev d = d_in;  // (the caller's copy may predate the plan)

@@ -240,14 +240,9 @@ int gb_voc_create(gb_ctx* ctx, int k, int L, int weighting, int scoring, uint32_
   if (e == cudaSuccess) e = cudaMemcpy(v->d_child, child_num, (size_t)n_nodes * 4, cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(v->d_weight, weight, (size_t)n_nodes * 4, cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(v->d_desc, desc32, (size_t)n_nodes * 32, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) {
-    static std::once_flag once[64];
-    std::call_once(once[ctx->device & 63], [&] {
-      e = cudaFuncSetAttribute(bow_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kSmemKeys * (int)sizeof(unsigned long long));
-    });
-  }
-  if (e != cudaSuccess) {
-    gb_set_error(ctx, "gb_voc_create -> %s", cudaGetErrorString(e));
+  const bool smem_ok = e == cudaSuccess && gb_func_setup(ctx, (const void*)bow_reduce_kernel, 2 * kSmemKeys * (int)sizeof(unsigned long long));
+  if (!smem_ok) {
+    gb_set_error(ctx, "gb_voc_create -> %s", e != cudaSuccess ? cudaGetErrorString(e) : "cannot set the shared-memory limit of the reduce kernel");
     cudaFree(v->d_child); cudaFree(v->d_weight); cudaFree(v->d_desc);
     delete v;
     return GB_ERR_CUDA;

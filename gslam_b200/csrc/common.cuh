@@ -64,6 +64,14 @@ int gb_stage_reserve(gb_ctx* ctx, size_t bytes);           // make sure the pinn
 void* gb_stage_alloc(gb_ctx* ctx, size_t bytes);           // bump-allocate from pinned staging (256-B aligned), or nullptr
 int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes);  // grow-only device buffer
 
+// Function attributes are per-function, per-DEVICE state shared by every ctx on the device: gb_func_setup sets kernel `fn`'s
+// dynamic shared-memory limit to `smem` bytes (GB_SMEM_OPTIN_MAX: the device's opt-in maximum less the kernel's static shared
+// memory) and, when `nonportable_cluster` is given, permits cluster sizes above 8, reporting there whether that worked.  Each
+// setting is made once per (device, function), under a lock, and a limit is never lowered: a value planned for one ctx's launch
+// cannot shrink under another's.  Returns whether the limit is set.
+constexpr int GB_SMEM_OPTIN_MAX = -1;
+bool gb_func_setup(gb_ctx* ctx, const void* fn, int smem, bool* nonportable_cluster = nullptr);
+
 #define GB_CUDA(ctx, call)                                                                              \
   do {                                                                                                  \
     cudaError_t e_ = (call);                                                                            \
@@ -107,6 +115,21 @@ static inline cudaError_t gb_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 #endif
+
+// Launch configuration of ONE thread-block cluster of `cluster` CTAs along x: for cudaLaunchKernelEx and
+// cudaOccupancyMaxActiveClusters.  (cfg points into the object: not copyable.)
+struct GbClusterConfig {
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute at[1];
+  GbClusterConfig(int cluster, dim3 block, size_t smem, cudaStream_t stream) {
+    cfg.gridDim = dim3(cluster); cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+  }
+  GbClusterConfig(const GbClusterConfig&) = delete;
+  GbClusterConfig& operator=(const GbClusterConfig&) = delete;
+};
 
 struct CtxLock {
   gb_ctx* c;

@@ -1,4 +1,6 @@
 // gslam_b200/csrc/ctx.cu — gb_ctx lifetime, error strings, pinned staging, timers, gb_features containers.
+#include <map>
+
 #include "common.cuh"
 
 static thread_local std::string g_tls_err = "";
@@ -46,6 +48,39 @@ int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes) {
   GB_CUDA(ctx, cudaMalloc(p, want));
   *cap = want;
   return GB_OK;
+}
+
+namespace {
+struct FuncSetup {
+  bool smem_ok = false;
+  int nonportable = 0;  // 0 not asked for yet, 1 permitted, -1 refused
+};
+std::mutex g_func_mu;
+std::map<std::pair<int, const void*>, FuncSetup> g_func_done;  // (device, kernel) -> what was set
+}  // namespace
+
+bool gb_func_setup(gb_ctx* ctx, const void* fn, int smem, bool* nonportable_cluster) {
+  std::lock_guard<std::mutex> lk(g_func_mu);
+  const auto key = std::make_pair(ctx->device, fn);
+  auto it = g_func_done.find(key);
+  if (it == g_func_done.end()) {
+    FuncSetup s;
+    s.smem_ok = true;
+    if (smem == GB_SMEM_OPTIN_MAX) {
+      cudaFuncAttributes fa{};
+      s.smem_ok = cudaFuncGetAttributes(&fa, fn) == cudaSuccess;
+      if (s.smem_ok) smem = ctx->max_smem_optin - (int)fa.sharedSizeBytes;
+    }
+    s.smem_ok = s.smem_ok && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess;
+    cudaGetLastError();  // (a refused attribute must not surface as the error of a later launch)
+    it = g_func_done.emplace(key, s).first;
+  }
+  if (nonportable_cluster && it->second.nonportable == 0) {
+    it->second.nonportable = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess ? 1 : -1;
+    cudaGetLastError();
+  }
+  if (nonportable_cluster) *nonportable_cluster = it->second.nonportable > 0;
+  return it->second.smem_ok;
 }
 
 extern void gb_orb_state_free(gb_ctx* ctx);

@@ -825,10 +825,9 @@ static int orb_prepare(gb_ctx* ctx, int w, int h, const gb_orb_cfg* cfg) {
       }
     }
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    GB_CUDA(ctx, cudaFuncSetAttribute(orb_describe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(DescSmem) * kDescWarps)));
-    attr_set = true;
+  if (!gb_func_setup(ctx, (const void*)orb_describe_kernel, (int)(sizeof(DescSmem) * kDescWarps))) {
+    gb_set_error(ctx, "gb_orb: cannot set the shared-memory limit of the describe kernel");
+    return GB_ERR_CUDA;
   }
   s->w = w; s->h = h; s->cfg = *cfg; s->valid = true;
   return GB_OK;
