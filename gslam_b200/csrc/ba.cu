@@ -940,20 +940,18 @@ __global__ void __launch_bounds__(1024) ba_install_pending_kernel(BaDev g) {
 //    in lane {0,1,2,-,3,4,5,-}[l] (lanes 3 and 7 duplicate rows 2 and 5).  Those lanes own element 6i+r of every CG vector;
 //    u = Minv r exchanges the camera's six residuals through a warp-local shared-memory tile (a camera never straddles
 //    warps: __syncwarp, no CTA barrier).
-//  * (gamma, delta) are reduced packed into ONE butterfly per warp (a in lanes 0-15, b in lanes 16-31); warp 0 alone folds the
-//    per-warp partials and runs the alpha/beta recurrences (one reciprocal) while the others wait at the barrier.
+//  * (gamma, delta) are reduced packed into ONE butterfly per warp (a in lanes 0-15, b in lanes 16-31); EVERY warp then folds
+//    the per-warp partials in warp order and runs the alpha/beta recurrences (one reciprocal) itself: identical operations on
+//    identical operands, so every thread holds the same bits and takes the same stop decision without a broadcast.
 //  * <= 48 active cameras run as 12 warps = 3 per sub-partition -> 168 registers per thread, enough for 7 columns per lane
-//    (block rows of <= 9 blocks) without spilling; the wide variant (<= 80 cameras) keeps 5 columns and reads the rest from
-//    the shared-memory copy of S.
-// An iteration = [partials | warp 0: scalars | element-wise recurrences, u = Minv r | u published | register mat-vec], three
-// barriers.
-template <int THREADS, int KC>
+//    (block rows of <= 9 blocks) without spilling; the wide variant (<= 80 cameras) keeps 5 columns.  Only graphs with a block
+//    row longer than the register columns (LONG_ROWS, chosen on the host) read the rest from the shared-memory copy of S.
+// An iteration = [partials | scalars, element-wise recurrences, u = Minv r | u published | register mat-vec], two barriers.
+template <int THREADS, int KC, bool LONG_ROWS>
 __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, double* __restrict__ buf, int maxit) {
   gb_pdl_launch_dependents();
   extern __shared__ __align__(16) double sm[];
   __shared__ double2 s_red[32];  // per-warp (gamma, delta) partials
-  __shared__ double s_scal[2][2];
-  __shared__ int s_flag[2];
   __shared__ int s_nact;
   constexpr int NW = THREADS / 32;
   static_assert(NW <= 32, "the fold handles at most 32 per-warp partials");
@@ -1032,6 +1030,16 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
   const int d = 6 * ci + row;
   const int b0 = cam_ok ? rowptr[ci] : 0, b1 = cam_ok ? rowptr[ci + 1] : 0;
   const int ncols = 6 * (b1 - b0);
+  // The mat-vec accumulates the camera's rows in a per-lane slot order chosen so that every butterfly exchange below sends and
+  // keeps FIXED slots (no selects in the loop): slots 0-2 hold the half this lane keeps after the first exchange, slots 3-5
+  // the same positions of the other half, and within a half lane {x0, x1, x2, x3} orders its rows {012, 102, 210, 201}.
+  const bool hi = (l8 & 4) != 0, mid = (l8 & 2) != 0, odd = (l8 & 1) != 0;
+  auto to_slots = [&](const double (&n)[6], double (&m)[6]) {  // one column, rows 0-5 -> slots 0-5
+    const double k0 = hi ? n[3] : n[0], k1 = hi ? n[4] : n[1], k2 = hi ? n[5] : n[2];  // the half this lane keeps
+    const double s0 = hi ? n[0] : n[3], s1 = hi ? n[1] : n[4], s2 = hi ? n[2] : n[5];  // the half it sends
+    m[0] = mid ? k2 : (odd ? k1 : k0); m[1] = odd ? k0 : k1; m[2] = mid ? (odd ? k1 : k0) : k2;
+    m[3] = mid ? s2 : (odd ? s1 : s0); m[4] = odd ? s0 : s1; m[5] = mid ? (odd ? s1 : s0) : s2;
+  };
   // this lane's columns of the block row: coefficients in registers (absent columns: zeros, reading the camera's own u)
   double cf[KC][6];
   int pidx[KC];
@@ -1041,8 +1049,10 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
     const bool ok = c < ncols;
     const int sblk = ok ? b0 + c / 6 : 0, a = ok ? c % 6 : 0;
     pidx[k] = ok ? 6 * col[sblk] + a : 6 * ci;
+    double n[6];
 #pragma unroll
-    for (int r = 0; r < 6; ++r) cf[k][r] = ok ? B[(size_t)sblk * 36 + r * 6 + a] : 0.0;
+    for (int r = 0; r < 6; ++r) n[r] = ok ? B[(size_t)sblk * 36 + r * 6 + a] : 0.0;
+    to_slots(n, cf[k]);
   }
   double mrow[6];  // this lane's row of the camera's Minv block (constant over the solve)
 #pragma unroll
@@ -1056,31 +1066,29 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
 #pragma unroll
     for (int k = 0; k < KC; ++k)
 #pragma unroll
-      for (int r = 0; r < 6; ++r) y[r] += cf[k][r] * pv[k];
-    for (int c = l8 + 8 * KC; c < ncols; c += 8) {  // block rows longer than the register cache: shared-memory copy
-      const int sblk = b0 + c / 6, a = c % 6;
-      const double pc = vu[6 * col[sblk] + a];
-      const double* Bc = B + (size_t)sblk * 36 + a;
+      for (int s = 0; s < 6; ++s) y[s] += cf[k][s] * pv[k];
+    if constexpr (LONG_ROWS) {
+      for (int c = l8 + 8 * KC; c < ncols; c += 8) {  // block rows longer than the register cache: shared-memory copy
+        const int sblk = b0 + c / 6, a = c % 6;
+        const double pc = vu[6 * col[sblk] + a];
+        const double* Bc = B + (size_t)sblk * 36 + a;
+        double n[6], m[6];
 #pragma unroll
-      for (int r = 0; r < 6; ++r) y[r] += Bc[r * 6] * pc;
+        for (int r = 0; r < 6; ++r) n[r] = Bc[r * 6];
+        to_slots(n, m);
+#pragma unroll
+        for (int s = 0; s < 6; ++s) y[s] += m[s] * pc;
+      }
     }
     // transposing butterfly over the 8 lanes of the camera: rows {0,1,2} go to lanes 0-3, rows {3,4,5} to lanes 4-7 ...
-    const bool hi = (l8 & 4) != 0, mid = (l8 & 2) != 0, odd = (l8 & 1) != 0;
     double v[3];
 #pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const double recv = __shfl_xor_sync(0xffffffffu, hi ? y[j] : y[3 + j], 4);
-      v[j] = (hi ? y[3 + j] : y[j]) + recv;
-    }
-    // ... then {first two} to lanes x0/x1 and {third} to lanes x2/x3 of each half ...
-    const double r1 = __shfl_xor_sync(0xffffffffu, mid ? v[0] : v[2], 2);
-    const double r2 = __shfl_xor_sync(0xffffffffu, v[1], 2);
-    const double t0 = (mid ? v[2] : v[0]) + r1;
-    const double t1 = v[1] + r2;  // (meaningful in the !mid lanes only)
+    for (int j = 0; j < 3; ++j) v[j] = y[j] + __shfl_xor_sync(0xffffffffu, y[3 + j], 4);
+    // ... then rows {0,1} of the half to lanes x0/x1 (t0 = x0's row 0, x1's row 1; t1 = the other) and row 2 to lanes x2/x3 ...
+    const double t0 = v[0] + __shfl_xor_sync(0xffffffffu, v[2], 2);
+    const double t1 = v[1] + __shfl_xor_sync(0xffffffffu, v[1], 2);  // (meaningful in the !mid lanes only)
     // ... and the last exchange finishes the sums (the two `mid` lanes of a half both end with the third row)
-    const double keep = mid ? t0 : (odd ? t1 : t0);
-    const double send = mid ? t0 : (odd ? t0 : t1);
-    return keep + __shfl_xor_sync(0xffffffffu, send, 1);
+    return t0 + __shfl_xor_sync(0xffffffffu, mid ? t0 : t1, 1);
   };
   // per-warp part of the fused deterministic reduction: lanes 0-15 fold a, lanes 16-31 fold b (ONE butterfly for both)
   auto warp_partials = [&](double a, double b) {
@@ -1100,6 +1108,8 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
     const double2 q01 = rc[0], q23 = rc[1], q45 = rc[2];
     return ((mrow[0] * q01.x + mrow[1] * q01.y) + (mrow[2] * q23.x + mrow[3] * q23.y)) + (mrow[4] * q45.x + mrow[5] * q45.y);
   };
+  // clock64 stamps of thread 0 (test hook gb_dbg_ba_pcg_profile): [7] setup cycles, then of iteration 3 [0] start, [1] scalars
+  // done, [2] u = Minv r stored, [3] after barrier (2) and the mat-vec, [4] partials stored; [6] the loop's end
 #define SP_STAMP(k) do { if (g.prof && tid == 0 && it == 3) g.prof[k] = clock64(); } while (0)
   if (g.prof && tid == 0) g.prof[7] = clock64() - t_start;
   // ---- Chronopoulos-Gear PCG (same recurrence as oracle/ba_ref.c::ba_pcg) ----
@@ -1110,60 +1120,60 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
   __syncthreads();  // u published
   wd = matvec();
   warp_partials(own ? rd * ud : 0.0, own ? wd * ud : 0.0);
-  // scalar recurrences: live in warp 0 only
+  // scalar recurrences: every thread runs them (same bits everywhere)
   const double tol2 = tol * tol;
   double gamma0 = 0.0, alpha_s = 0.0, beta_s = 0.0, inv_alpha = 0.0, inv_gamma = 0.0;
   int iters = 0;
+  // Two barriers per iteration suffice.  s_red: a warp writes its partials of round `it` after barrier (2) of iteration it-1 and
+  // every warp reads them after barrier (1) of iteration `it`; the next write comes after barrier (2) of iteration `it`, which no
+  // warp passes before it has finished its fold.  vu: written before barrier (2), read by the mat-vec after it; the next write
+  // comes after barrier (1) of the following iteration, which no warp passes before its mat-vec is done.  vr is warp-local
+  // (__syncwarp inside precond) and is rewritten only after both barriers.
   for (int it = 0;; ++it) {
     SP_STAMP(0);
-    __syncthreads();  // the partials of round `it` are in s_red (round 0: the initial gamma, delta; round k: iteration k-1)
-    if (warp == 0) {
-      double gn = 0.0, dl = 0.0;  // fixed-order fold of the per-warp partials (broadcast loads, two independent chains)
+    __syncthreads();  // (1) the partials of round `it` are in s_red (round 0: the initial gamma, delta; round k: iteration k-1)
+    double gn = 0.0, dl = 0.0;  // fixed-order fold of the per-warp partials (broadcast loads, two independent chains)
 #pragma unroll
-      for (int w = 0; w < NW; ++w) { const double2 t = s_red[w]; gn += t.x; dl += t.y; }
-      // alpha = gn/den, 1/alpha = den/gn and 1/gn from ONE reciprocal: t = 1/(gn*den) (a DDIV is ~113 clk and three of them do
-      // not overlap); the guarded fallback covers products outside the double range
-      auto scalars = [&](double den) {
-        const double t = __drcp_rn(gn * den);
-        if (t > 0.0 && t < 1.0e300) {
-          const double inv_gn = den * t, inv_den = gn * t;
-          alpha_s = gn * inv_den; inv_alpha = den * inv_gn; inv_gamma = inv_gn;
-        } else {
-          alpha_s = gn / den; inv_alpha = den / gn; inv_gamma = 1.0 / gn;
-        }
-      };
-      bool stop;
-      if (it == 0) {
-        gamma0 = gn;
-        stop = !(gamma0 > 0.0) || !(dl > 0.0) || maxit <= 0;
-        if (!stop) scalars(dl);
+    for (int w = 0; w < NW; ++w) { const double2 t = s_red[w]; gn += t.x; dl += t.y; }
+    // alpha = gn/den, 1/alpha = den/gn and 1/gn from ONE reciprocal: t = 1/(gn*den) (a DDIV is ~113 clk and three of them do
+    // not overlap); the guarded fallback covers products outside the double range
+    auto scalars = [&](double den) {
+      const double t = __drcp_rn(gn * den);
+      if (t > 0.0 && t < 1.0e300) {
+        const double inv_gn = den * t, inv_den = gn * t;
+        alpha_s = gn * inv_den; inv_alpha = den * inv_gn; inv_gamma = inv_gn;
       } else {
-        iters = it;
-        stop = !(gn > 0.0) || gn < tol2 * gamma0;
-        if (!stop) {
-          // beta = gn/gamma, alpha = gn/(dl - beta*gn/alpha_prev) with the reciprocals of gamma and alpha carried along
-          beta_s = gn * inv_gamma;
-          const double den = dl - beta_s * (gn * inv_alpha);
-          stop = !(den > 0.0);
-          if (!stop) scalars(den);
-        }
-        stop = stop || it >= maxit;
+        alpha_s = gn / den; inv_alpha = den / gn; inv_gamma = 1.0 / gn;
       }
-      if (lane == 0) { s_scal[it & 1][0] = alpha_s; s_scal[it & 1][1] = beta_s; s_flag[it & 1] = stop ? 1 : 0; }
+    };
+    bool stop;
+    if (it == 0) {
+      gamma0 = gn;
+      stop = !(gamma0 > 0.0) || !(dl > 0.0) || maxit <= 0;
+      if (!stop) scalars(dl);
+    } else {
+      iters = it;
+      stop = !(gn > 0.0) || gn < tol2 * gamma0;
+      if (!stop) {
+        // beta = gn/gamma, alpha = gn/(dl - beta*gn/alpha_prev) with the reciprocals of gamma and alpha carried along
+        beta_s = gn * inv_gamma;
+        const double den = dl - beta_s * (gn * inv_alpha);
+        stop = !(den > 0.0);
+        if (!stop) scalars(den);
+      }
+      stop = stop || it >= maxit;
     }
     SP_STAMP(1);
-    __syncthreads();  // scalars of round `it` published
-    if (s_flag[it & 1]) break;
-    const double alpha = s_scal[it & 1][0], beta = s_scal[it & 1][1];
+    if (stop) break;
     // element-wise recurrences, registers only (duplicate lanes compute duplicates)
-    pd = ud + beta * pd;
-    sd = wd + beta * sd;
-    xd += alpha * pd;
-    rd -= alpha * sd;
+    pd = ud + beta_s * pd;
+    sd = wd + beta_s * sd;
+    xd += alpha_s * pd;
+    rd -= alpha_s * sd;
     ud = precond(rd);
-    if (own) vu[d] = ud;  // (every mat-vec read of the previous u happened before the two barriers above)
+    if (own) vu[d] = ud;
     SP_STAMP(2);
-    __syncthreads();  // u published
+    __syncthreads();  // (2) u published
     wd = matvec();
     SP_STAMP(3);
     warp_partials(own ? rd * ud : 0.0, own ? wd * ud : 0.0);
@@ -1179,9 +1189,10 @@ __global__ void __launch_bounds__(THREADS, 1) ba_pcg_sparse_kernel(BaDev g, doub
 }
 constexpr int kSpSmallCams = 48;     // active cameras of the 12-warp variant (168 registers, 7 register columns per lane)
 constexpr int kSpMaxCams = 80;       // active cameras of the 20-warp variant (96 registers, 5 register columns per lane)
+constexpr int kSpSmallCols = 7, kSpLargeCols = 5;
 constexpr int kSpSmallThreads = 8 * kSpSmallCams, kSpLargeThreads = 8 * kSpMaxCams;
-#define BA_SPARSE_SMALL ba_pcg_sparse_kernel<kSpSmallThreads, 7>
-#define BA_SPARSE_LARGE ba_pcg_sparse_kernel<kSpLargeThreads, 5>
+#define BA_SPARSE_SMALL(long_rows) ba_pcg_sparse_kernel<kSpSmallThreads, kSpSmallCols, long_rows>
+#define BA_SPARSE_LARGE(long_rows) ba_pcg_sparse_kernel<kSpLargeThreads, kSpLargeCols, long_rows>
 
 // ---- K7b (local BA): block-Jacobi PCG inside ONE thread-block cluster ------------------------------------------------------
 // Each CTA of the cluster keeps a block-row slice of the (damped) reduced camera matrix S resident in its shared memory for the
@@ -1433,8 +1444,10 @@ static void ba_pick_pcg(gb_ctx* ctx, gb_ba_graph* g) {
   g->pcg_sparse = false;
   const int nc = g->d.nc, n6 = g->d.n6;
   bool cluster16_ok = false;
-  bool smem_ok = gb_func_setup(ctx, (const void*)BA_SPARSE_SMALL, GB_SMEM_OPTIN_MAX);
-  smem_ok = gb_func_setup(ctx, (const void*)BA_SPARSE_LARGE, GB_SMEM_OPTIN_MAX) && smem_ok;
+  bool smem_ok = true;
+  for (const void* f : {(const void*)BA_SPARSE_SMALL(false), (const void*)BA_SPARSE_SMALL(true), (const void*)BA_SPARSE_LARGE(false),
+                        (const void*)BA_SPARSE_LARGE(true)})
+    smem_ok = gb_func_setup(ctx, f, GB_SMEM_OPTIN_MAX) && smem_ok;
   smem_ok = gb_func_setup(ctx, (const void*)ba_pcg_cluster_kernel, GB_SMEM_OPTIN_MAX, &cluster16_ok) && smem_ok;
   if (nc > 0 && g->pcg_nact <= kSpMaxCams && g->d.s_nnzb > 0) {
     const size_t smem = ((size_t)g->d.s_nnzb * 36 + (size_t)nc * 36 + 3 * (size_t)n6) * sizeof(double) + (2 * (size_t)nc + 1 + g->d.s_nnzb) * sizeof(int) + 64;
@@ -2079,10 +2092,14 @@ int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
 
 extern "C" {
 
-// single-CTA block-sparse PCG, in the variant that fits the graph's active cameras (pdl: programmatic dependent launch)
+// single-CTA block-sparse PCG, in the variant that fits the graph's active cameras and its longest block row of S (the
+// shared-memory path for columns beyond the registers is compiled in only where a row needs it; pdl: programmatic dependent
+// launch)
 static int ba_pcg_sparse_launch(gb_ctx* ctx, gb_ba_graph* g, double* buf, bool pdl) {
   const bool small = g->pcg_nact <= kSpSmallCams;
-  void (*kernel)(BaDev, double*, int) = small ? BA_SPARSE_SMALL : BA_SPARSE_LARGE;
+  const bool long_rows = 6 * g->pcg_max_row_blocks > 8 * (small ? kSpSmallCols : kSpLargeCols);
+  void (*kernel)(BaDev, double*, int) = small ? (long_rows ? BA_SPARSE_SMALL(true) : BA_SPARSE_SMALL(false))
+                                              : (long_rows ? BA_SPARSE_LARGE(true) : BA_SPARSE_LARGE(false));
   const dim3 block(small ? kSpSmallThreads : kSpLargeThreads);
   const int maxit = (int)g->opt.pcg_max_iters;
   if (pdl) GB_CUDA(ctx, gb_launch_pdl(kernel, dim3(1), block, g->pcg_sparse_smem, ctx->stream, g->d, buf, maxit));
