@@ -455,11 +455,12 @@ class Comm:
     """A rank of the multi-GPU communicator (gb_comm): NCCL under the C-ABI.  `unique_id` is the 128 bytes rank 0 obtained from
     Comm.unique_id() and the host distributed (torch.distributed broadcast in bench.py / tests)."""
 
-    def __init__(self, ctx: Context, world: int = 1, rank: int = 0, unique_id: bytes | None = None):
+    def __init__(self, ctx: Context, world: int = 1, rank: int = 0, unique_id: bytes | None = None, _handle=None):
         self.ctx = ctx
-        h = C.c_void_p()
-        buf = (C.c_uint8 * 128).from_buffer_copy(unique_id) if unique_id is not None else None
-        ctx._check(ctx._lib.gb_comm_create(ctx._h, world, rank, C.cast(buf, C.c_void_p) if buf is not None else None, C.byref(h)))
+        h = C.c_void_p(_handle) if _handle is not None else C.c_void_p()
+        if _handle is None:
+            buf = (C.c_uint8 * 128).from_buffer_copy(unique_id) if unique_id is not None else None
+            ctx._check(ctx._lib.gb_comm_create(ctx._h, world, rank, C.cast(buf, C.c_void_p) if buf is not None else None, C.byref(h)))
         self._h = h
         self.rank, self.world = rank, world
 
@@ -503,22 +504,55 @@ class ShardedBAGraph(BAGraph):
         self.ctx._check(self.ctx._lib.gb_ba_shard_solve(self.comm._h, self._h, C.byref(o), C.byref(r)))
         return r
 
+    def dbg_shard_reduced(self, cfg: OptimzeConfig | None = None, allreduce: bool = False):
+        """(S dense 6N x 6N undamped, g~, diag U, cost) of one iteration at the current estimate (test hook); with `allreduce` a
+        collective that every rank calls."""
+        n6 = 6 * self.n_cams
+        S = np.zeros((n6, n6)); gt = np.zeros(n6); dU = np.zeros(n6); cost = np.zeros(1)
+        o = (cfg or OptimzeConfig()).to_c()
+        self.ctx._check(self.ctx._lib.gb_dbg_ba_shard_reduced(self.comm._h, self._h, C.byref(o), int(allreduce), ptr(S), ptr(gt), ptr(dU),
+                                                              ptr(cost)))
+        return S, gt, dU, float(cost[0])
 
-def ba_solve_multi(ctxs, pb: BAProblem, cfg: OptimzeConfig | None = None) -> capi.BaResult:
-    """One process, len(ctxs) GPUs: gb_comm_create_all + gb_ba_solve_multi (what the optimizer plugin does for b200.devices)."""
+
+def local_group(ctx: Context, world: int):
+    """A loopback communicator of `world` ranks on ctx's device (test hook gb_dbg_comm_create_local): -> (ctxs, comms).  ctxs[0] is
+    `ctx`; the others share its stream.  Close the comms, then ctxs[1:], before `ctx`."""
+    L = ctx._lib
+    hc = (C.c_void_p * world)()
+    hm = (C.c_void_p * world)()
+    rc = L.gb_dbg_comm_create_local(ctx._h, world, hc, hm)
+    if rc != capi.GB_OK:
+        raise GbError(rc, L.gb_last_error(None).decode())
+    ctxs = [ctx]
+    for r in range(1, world):
+        c = Context.__new__(Context)
+        c._lib, c._h, c.device = L, C.c_void_p(hc[r]), ctx.device
+        ctxs.append(c)
+    return ctxs, [Comm(ctxs[r], world, r, _handle=hm[r]) for r in range(world)]
+
+
+def ba_solve_multi(ctxs, pb: BAProblem, cfg: OptimzeConfig | None = None, comms=None) -> capi.BaResult:
+    """One process, len(ctxs) GPUs: gb_comm_create_all + gb_ba_solve_multi (what the optimizer plugin does for b200.devices).  With
+    `comms` (Comm objects, e.g. from local_group) those communicators are used instead, and the caller keeps them."""
     L = capi.lib()
     n = len(ctxs)
-    hs = (C.c_void_p * n)(*[c._h for c in ctxs])
-    comms = (C.c_void_p * n)()
-    ctxs[0]._check(L.gb_comm_create_all(n, hs, comms))
+    own = comms is None
+    if own:
+        hs = (C.c_void_p * n)(*[c._h for c in ctxs])
+        hm = (C.c_void_p * n)()
+        ctxs[0]._check(L.gb_comm_create_all(n, hs, hm))
+    else:
+        hm = (C.c_void_p * n)(*[m._h.value for m in comms])
     try:
         c, keep = _problem_c(pb)
         o = (cfg or OptimzeConfig()).to_c(); r = capi.BaResult()
-        ctxs[0]._check(L.gb_ba_solve_multi(n, comms, C.byref(c), C.byref(o), C.byref(r)))
+        ctxs[0]._check(L.gb_ba_solve_multi(n, hm, C.byref(c), C.byref(o), C.byref(r)))
         return r
     finally:
-        for k in range(n):
-            L.gb_comm_destroy(comms[k])
+        if own:
+            for k in range(n):
+                L.gb_comm_destroy(hm[k])
 
 class Optimizer:
     """Mirror of GSLAM::Optimizer (Optimizer.h:184-253): bool returns, graph / pose updated in place, `_config` public."""

@@ -142,6 +142,8 @@ _DEBUG_SIGNATURES = [
     ("gb_dbg_pnp_p3p_host", C.c_int, [_VP, _VP, _VP]),
     ("gb_dbg_pnp_minimal_host", C.c_int, [C.c_int, _VP, _VP, C.c_double, C.c_double, C.c_int, C.c_uint64, _VP, C.POINTER(PnpStats)]),
     ("gb_dbg_ba_shard_bounds", C.c_int, [C.c_int, C.c_int, _VP, C.c_int, _VP]),
+    ("gb_dbg_comm_create_local", C.c_int, [_VP, C.c_int, C.POINTER(_VP), C.POINTER(_VP)]),
+    ("gb_dbg_ba_shard_reduced", C.c_int, [_VP, _VP, C.POINTER(BaOptions), C.c_int, _VP, _VP, _VP, _VP]),
     ("gb_dbg_popc_peak", C.c_int, [_VP, C.POINTER(C.c_double)]),
     ("gb_dbg_orb_level_size", C.c_int, [C.c_int, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
 ]

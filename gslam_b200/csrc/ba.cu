@@ -2063,11 +2063,16 @@ static int ba_red_blocks(const gb_ctx* ctx, int n) { return std::max(1, std::min
 // ---- one LM iteration on the COMPACT reduced layout rbuf = [Sb (nnzb x 36) | g~ | diag U | cost | pad] ------------------------------
 // (large graphs on one GPU and every rank of the landmark-sharded solve: with a communicator, what the collective sums is the shard's
 // contribution to the reduced system and to the candidate cost)
-int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
+static BaDev ba_compact_dev(const gb_ba_graph* g) {
   BaDev d = g->d;
   d.Sb = g->rbuf;
   d.r_gt = (size_t)d.s_nnzb * 36;
   d.vinv_in_sweep = ba_sweep_is_large(g) ? 0 : 1;
+  return d;
+}
+
+int ba_compact_reduce(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
+  const BaDev d = ba_compact_dev(g);
   cudaStream_t s = ctx->stream;
   GB_CHECK(ba_launch_sweep(ctx, g, d, s, 3));
   {
@@ -2081,6 +2086,12 @@ int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
     ba_schur_blocks_kernel<<<d.s_nupper, 128, 0, s>>>(d, g->rbuf); GB_LAUNCH_CHECK(ctx);
   }
   if (comm) GB_CHECK(gb_comm_allreduce_sum_f64(comm, g->rbuf, g->rbuf_doubles));
+  return GB_OK;
+}
+
+int ba_compact_step(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
+  const BaDev d = ba_compact_dev(g);
+  cudaStream_t s = ctx->stream;
   GB_CHECK(ba_pcg_bcsr_launch(ctx, g, g->rbuf));
   if (d.np > 0) { ba_backsub_cost_kernel<<<gb_div_up(d.np * kLpp, 128), 128, 0, s>>>(d); GB_LAUNCH_CHECK(ctx); }
   ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np), kRedThreads, 0, s>>>(d, d.cost_pt_new, d.np, g->d_cost); GB_LAUNCH_CHECK(ctx);
@@ -2088,6 +2099,11 @@ int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
   const int n = std::max(std::max(d.nc * 12, d.np * 3), 1);
   ba_commit_apply_kernel<<<gb_div_up(n, 256), 256, 0, s>>>(d, g->rbuf, g->d_cost); GB_LAUNCH_CHECK(ctx);
   return GB_OK;
+}
+
+int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
+  GB_CHECK(ba_compact_reduce(ctx, g, comm));
+  return ba_compact_step(ctx, g, comm);
 }
 
 extern "C" {

@@ -14,7 +14,8 @@
 // The collective is NCCL, bound at run time with dlopen (the library loads and the single-GPU paths work without NCCL); two
 // front ends share the engine: one process per GPU (gb_comm_create from a unique id the host distributes -- bench.py under
 // torchrun) and one process driving N GPUs (gb_comm_create_all + gb_ba_solve_multi, one host thread per device -- what the
-// libgslam_optimizer.so plugin uses when the svar option b200.devices lists several devices).
+// libgslam_optimizer.so plugin uses when the svar option b200.devices lists several devices).  A loopback transport (test hook
+// gb_dbg_comm_create_local) runs the same engine with several ranks on one device.
 #include "ba_internal.cuh"
 
 #include <dlfcn.h>
@@ -22,6 +23,7 @@
 #include <algorithm>
 #include <chrono>
 #include <cmath>
+#include <condition_variable>
 #include <thread>
 
 namespace {
@@ -68,13 +70,88 @@ NcclApi& nccl() {
   return api;
 }
 
+// ---- loopback transport (test hook gb_dbg_comm_create_local): `world` ranks on ONE device whose contexts share one stream ------
+// A host rendezvous per collective; the last rank to arrive enqueues one kernel that sums the buffers in rank order and writes the
+// sum into every buffer, then releases the others.  So every rank gets the same bits (as with NCCL), no events are needed, and
+// the ranks' kernels never run concurrently (one rank's cooperative-grid PCG never competes with another's for residency).
+constexpr int kLoopbackMaxWorld = 16;
+constexpr auto kLoopbackTimeout = std::chrono::seconds(120);
+
+struct LoopbackBufs {
+  double* p[kLoopbackMaxWorld];
+};
+
+__global__ void loopback_sum_kernel(LoopbackBufs b, int world, size_t n) {
+  for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (size_t)gridDim.x * blockDim.x) {
+    double s = b.p[0][k];
+    for (int r = 1; r < world; ++r) s += b.p[r][k];
+    for (int r = 0; r < world; ++r) b.p[r][k] = s;
+  }
+}
+
+struct LoopbackGroup {
+  int world = 0, live = 0;  // live: communicators of the group not destroyed yet
+  cudaStream_t stream = nullptr;
+  int sm_count = 0;
+  std::mutex mu;
+  std::condition_variable cv;
+  unsigned long long gen = 0;  // collectives completed
+  int arrived = 0;
+  size_t n = 0;
+  bool n_mismatch = false;
+  LoopbackBufs bufs{};
+  bool here[kLoopbackMaxWorld] = {};
+  int rc = GB_OK;  // outcome of the last completed collective, and its message
+  std::string err;
+};
+
 }  // namespace
 
 struct gb_comm {
   gb_ctx* ctx = nullptr;
   ncclComm_t comm = nullptr;  // null when world == 1
+  LoopbackGroup* loop = nullptr;  // the loopback transport instead of NCCL
   int rank = 0, world = 1;
 };
+
+static int loopback_allreduce(gb_comm* c, double* d_buf, size_t n) {
+  LoopbackGroup& G = *c->loop;
+  std::unique_lock<std::mutex> lk(G.mu);
+  const unsigned long long gen = G.gen;
+  if (G.arrived == 0) { G.n = n; G.n_mismatch = false; }
+  else if (n != G.n) G.n_mismatch = true;
+  G.bufs.p[c->rank] = d_buf;
+  G.here[c->rank] = true;
+  if (++G.arrived == G.world) {
+    G.rc = GB_OK;
+    G.err.clear();
+    if (G.n_mismatch) {
+      G.rc = GB_ERR_INVALID;
+      G.err = "gb_comm (loopback): the ranks passed different lengths to one all-reduce";
+    } else if (G.n > 0) {
+      const int blocks = (int)std::min<size_t>((G.n + 255) / 256, (size_t)G.sm_count * 8);
+      loopback_sum_kernel<<<blocks, 256, 0, G.stream>>>(G.bufs, G.world, G.n);
+      c->ctx->launches++;
+      const cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) { G.rc = GB_ERR_CUDA; G.err = std::string("gb_comm (loopback): sum kernel -> ") + cudaGetErrorString(e); }
+    }
+    G.arrived = 0;
+    for (int r = 0; r < G.world; ++r) G.here[r] = false;
+    ++G.gen;
+    G.cv.notify_all();
+  } else if (!G.cv.wait_for(lk, kLoopbackTimeout, [&] { return G.gen != gen; })) {
+    std::string missing;
+    for (int r = 0; r < G.world; ++r)
+      if (!G.here[r]) missing += (missing.empty() ? "" : ", ") + std::to_string(r);
+    G.here[c->rank] = false;  // (withdraw: a late rank must not complete a collective this rank left)
+    --G.arrived;
+    gb_set_error(c->ctx, "gb_comm (loopback): rank %d waited %d s at an all-reduce of %zu doubles; rank(s) %s never arrived", c->rank,
+                 (int)kLoopbackTimeout.count(), n, missing.c_str());
+    return GB_ERR_CUDA;
+  }
+  if (G.rc != GB_OK) gb_set_error(c->ctx, "%s", G.err.c_str());
+  return G.rc;
+}
 
 #define GB_NCCL(ctx, call)                                                                              \
   do {                                                                                                  \
@@ -136,6 +213,14 @@ int gb_comm_create_all(int n_dev, gb_ctx* const* ctxs, gb_comm** out) {
 
 int gb_comm_destroy(gb_comm* c) {
   if (!c) return GB_OK;
+  if (c->loop) {
+    bool last;
+    {
+      std::lock_guard<std::mutex> lk(c->loop->mu);
+      last = --c->loop->live == 0;
+    }
+    if (last) delete c->loop;
+  }
   if (c->comm) {
     CtxLock lk(c->ctx);
     cudaStreamSynchronize(c->ctx->stream);
@@ -150,7 +235,12 @@ int gb_comm_world(const gb_comm* c) { return c ? c->world : -1; }
 
 int gb_comm_allreduce_sum_f64(gb_comm* c, double* d_buf, size_t n) {
   if (!c || !d_buf) return GB_ERR_INVALID;
-  if (c->world == 1 || n == 0) return GB_OK;
+  if (c->world == 1) return GB_OK;
+  if (c->loop) {  // (n == 0 too: a collective every rank must reach)
+    CtxLock lk(c->ctx);
+    return loopback_allreduce(c, d_buf, n);
+  }
+  if (n == 0) return GB_OK;
   CtxLock lk(c->ctx);
   GB_NCCL(c->ctx, nccl().AllReduce(d_buf, d_buf, n, kNcclFloat64, kNcclSum, c->comm, c->ctx->stream));
   return GB_OK;
@@ -239,6 +329,65 @@ int gb_ba_solve_multi(int n_dev, gb_comm* const* comms, gb_ba_problem* pb, const
     *res = rr[0];
     for (int r = 1; r < n_dev; ++r) res->gpu_ms = std::max(res->gpu_ms, rr[r].gpu_ms);
   }
+  return GB_OK;
+}
+
+// ---- test hooks ---------------------------------------------------------------------------------------------------------------
+// A loopback group of `world` ranks on base's device, for testing the sharded engine on one GPU: rank 0 runs on `base`, ranks
+// 1..world-1 on new contexts that share base's stream (ctxs_out[r]; the caller destroys them before `base`).  Separate contexts are
+// needed because gb_ba_shard_solve holds its ctx lock for the whole LM loop.  NCCL is not involved.
+GB_API int gb_dbg_comm_create_local(gb_ctx* base, int world, gb_ctx** ctxs_out, gb_comm** comms_out) {
+  if (!base || world < 1 || world > kLoopbackMaxWorld || !ctxs_out || !comms_out) return GB_ERR_INVALID;
+  for (int r = 0; r < world; ++r) { ctxs_out[r] = nullptr; comms_out[r] = nullptr; }
+  ctxs_out[0] = base;
+  for (int r = 1; r < world; ++r) {
+    const int rc = gb_ctx_create_on_stream(base->device, base->stream, &ctxs_out[r]);
+    if (rc != GB_OK) {
+      for (int k = 1; k < r; ++k) { gb_ctx_destroy(ctxs_out[k]); ctxs_out[k] = nullptr; }
+      ctxs_out[0] = nullptr;
+      return rc;
+    }
+  }
+  LoopbackGroup* grp = new LoopbackGroup();
+  grp->world = grp->live = world;
+  grp->stream = base->stream;
+  grp->sm_count = base->sm_count;
+  for (int r = 0; r < world; ++r) {
+    comms_out[r] = new gb_comm();
+    comms_out[r]->ctx = ctxs_out[r]; comms_out[r]->rank = r; comms_out[r]->world = world; comms_out[r]->loop = grp;
+  }
+  return GB_OK;
+}
+
+// The compact reduced system of ONE LM iteration of a shard at its current estimate: begin, then the first half of the iteration
+// (sweep, Schur complement of the shard's landmarks into rbuf) and, when `allreduce` is set, the all-reduce (a collective: every
+// rank calls it).  S (6N x 6N, dense, undamped), g~, diag U (n6 each) and the cost, each where non-null.
+GB_API int gb_dbg_ba_shard_reduced(gb_comm* c, gb_ba_graph* g, const gb_ba_options* opt, int allreduce, double* S, double* gt,
+                                   double* diagU, double* cost) {
+  if (!c || !g) return GB_ERR_INVALID;
+  gb_ctx* ctx = c->ctx;
+  CtxLock lk(ctx);
+  if (!g->pcg_bcsr || !g->rbuf) { gb_set_error(ctx, "gb_dbg_ba_shard_reduced: the graph has no block-CSR reduced system"); return GB_ERR_INVALID; }
+  if (g->shard_world != c->world || g->shard_rank != c->rank) { gb_set_error(ctx, "gb_dbg_ba_shard_reduced: graph / communicator mismatch"); return GB_ERR_INVALID; }
+  GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
+  GB_CHECK(ba_compact_reduce(ctx, g, allreduce ? c : nullptr));
+  const BaDev& d = g->d;
+  const size_t n6 = d.n6, nnzb = d.s_nnzb;
+  std::vector<double> rb(g->rbuf_doubles);
+  std::vector<int> brow(nnzb), col(nnzb);
+  GB_CUDA(ctx, cudaMemcpyAsync(rb.data(), g->rbuf, rb.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(brow.data(), d.s_brow, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(col.data(), d.s_col, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (S) {
+    memset(S, 0, n6 * n6 * sizeof(double));
+    for (size_t blk = 0; blk < nnzb; ++blk)
+      for (int k = 0; k < 36; ++k) S[(6 * (size_t)brow[blk] + k / 6) * n6 + 6 * (size_t)col[blk] + k % 6] = rb[36 * blk + k];
+  }
+  const double* tail = rb.data() + 36 * nnzb;
+  if (gt) memcpy(gt, tail, n6 * sizeof(double));
+  if (diagU) memcpy(diagU, tail + n6, n6 * sizeof(double));
+  if (cost) *cost = tail[2 * n6];
   return GB_OK;
 }
 

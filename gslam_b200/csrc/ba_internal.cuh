@@ -99,6 +99,10 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
 // needed) + Schur blocks, block-CSR PCG, back-substitution + candidate cost, LM accept / reject + install.  A non-null `comm`
 // all-reduces the reduced system and the candidate cost of this landmark shard before they are used.
 int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
+// its two halves: ba_compact_reduce = sweep + Schur complement of this graph's landmarks into rbuf (+ the all-reduce);
+// ba_compact_step = PCG, back-substitution + candidate cost (+ its all-reduce), LM accept / reject
+int ba_compact_reduce(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
+int ba_compact_step(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
 
 // ---- ba_pose.cu -------------------------------------------------------------------------------------------------------------
 // pose-graph terms (SE3Edge / GPSEdge, Optimizer.h:127-148) on the stepwise dense-layout solver path

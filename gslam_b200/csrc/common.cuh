@@ -20,6 +20,7 @@ struct gb_ctx {
   int sm_count = 132;
   int max_smem_optin = 0;
   cudaStream_t stream = nullptr;
+  bool owns_stream = true;                    // false: `stream` belongs to another ctx (gb_ctx_create_on_stream)
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // gb_timer_*
   cudaEvent_t evs = nullptr, eve = nullptr;   // internal (gb_ba_result.gpu_ms)
   cudaEvent_t ev_x = nullptr;                 // gb_ctx_wait_for (cross-ctx ordering)
@@ -60,6 +61,8 @@ struct gb_features {
 };
 
 void gb_set_error(gb_ctx* ctx, const char* fmt, ...);
+// A ctx on `device` that enqueues on `stream`, which another ctx owns and must outlive it (gb_ctx_destroy leaves it alone).
+int gb_ctx_create_on_stream(int device, cudaStream_t stream, gb_ctx** out);
 int gb_stage_reserve(gb_ctx* ctx, size_t bytes);           // make sure the pinned staging holds >= bytes
 void* gb_stage_alloc(gb_ctx* ctx, size_t bytes);           // bump-allocate from pinned staging (256-B aligned), or nullptr
 int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes);  // grow-only device buffer

@@ -103,16 +103,25 @@ int gb_device_count(int* n) {
   return GB_OK;
 }
 
-static int ctx_create_impl(int device, int high_priority, gb_ctx** out);
+static int ctx_create_impl(int device, int high_priority, cudaStream_t borrowed, gb_ctx** out);
 
-int gb_ctx_create(int device, gb_ctx** out) { return ctx_create_impl(device, 0, out); }
+int gb_ctx_create(int device, gb_ctx** out) { return ctx_create_impl(device, 0, nullptr, out); }
 
 // A ctx whose stream has the device's greatest priority: the block scheduler hands free SM slots to its CTAs first.  For the
 // mapping ctx of a tracking/mapping pair: the few-CTA local-BA kernels then do not queue behind the thousands of CTAs of the
 // tracking ctx's FAST / describe grids (without it the two streams barely overlap).
-int gb_ctx_create_priority(int device, int high_priority, gb_ctx** out) { return ctx_create_impl(device, high_priority, out); }
+int gb_ctx_create_priority(int device, int high_priority, gb_ctx** out) { return ctx_create_impl(device, high_priority, nullptr, out); }
 
-static int ctx_create_impl(int device, int high_priority, gb_ctx** out) {
+}  // extern "C"
+
+int gb_ctx_create_on_stream(int device, cudaStream_t stream, gb_ctx** out) {
+  if (!stream) return GB_ERR_INVALID;
+  return ctx_create_impl(device, 0, stream, out);
+}
+
+extern "C" {
+
+static int ctx_create_impl(int device, int high_priority, cudaStream_t borrowed, gb_ctx** out) {
   if (!out) return GB_ERR_INVALID;
   *out = nullptr;
   int n = 0;
@@ -127,7 +136,10 @@ static int ctx_create_impl(int device, int high_priority, gb_ctx** out) {
   gb_ctx* ctx = new gb_ctx();
   ctx->device = device;
   cudaError_t e = cudaSetDevice(device);
-  if (e == cudaSuccess) {
+  if (e == cudaSuccess && borrowed) {
+    ctx->stream = borrowed;
+    ctx->owns_stream = false;
+  } else if (e == cudaSuccess) {
     int lo = 0, hi = 0;  // (numerically lower = higher priority)
     if (high_priority && cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess) e = cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, hi);
     else e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
@@ -143,7 +155,7 @@ static int ctx_create_impl(int device, int high_priority, gb_ctx** out) {
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     if (ctx->evs) cudaEventDestroy(ctx->evs);
     if (ctx->eve) cudaEventDestroy(ctx->eve);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
+    if (ctx->stream && ctx->owns_stream) cudaStreamDestroy(ctx->stream);
     if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
     delete ctx;
   };
@@ -179,7 +191,7 @@ int gb_ctx_destroy(gb_ctx* ctx) {
     cudaEventDestroy(ctx->evs);
     cudaEventDestroy(ctx->eve);
     if (ctx->ev_x) cudaEventDestroy(ctx->ev_x);
-    cudaStreamDestroy(ctx->stream);
+    if (ctx->owns_stream) cudaStreamDestroy(ctx->stream);
   }
   delete ctx;
   return GB_OK;
