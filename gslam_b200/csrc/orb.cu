@@ -800,16 +800,20 @@ static int orb_prepare(gb_ctx* ctx, int w, int h, const gb_orb_cfg* cfg) {
   {  // TMA tensor maps: one per level over the padded-pitch buffer, u8, box = the FAST input tile; out-of-image reads give 0
     typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static EncodeFn encode = nullptr;
-    if (!encode) {
+    // looked up once per process; contexts on other threads may reach here at the same time (a function-local static is
+    // initialised exactly once, the others wait for it)
+    static const EncodeFn encode = []() -> EncodeFn {
       void* fn = nullptr;
       cudaDriverEntryPointQueryResult qr;
-      if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) != cudaSuccess || qr != cudaDriverEntryPointSuccess || !fn) {
+      if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) != cudaSuccess || qr != cudaDriverEntryPointSuccess) {
         cudaGetLastError();
-        gb_set_error(ctx, "gb_orb: cuTensorMapEncodeTiled is not available from this driver (the FAST kernel stages its tiles with TMA)");
-        return GB_ERR_CUDA;
+        fn = nullptr;
       }
-      encode = (EncodeFn)fn;
+      return (EncodeFn)fn;
+    }();
+    if (!encode) {
+      gb_set_error(ctx, "gb_orb: cuTensorMapEncodeTiled is not available from this driver (the FAST kernel stages its tiles with TMA)");
+      return GB_ERR_CUDA;
     }
     memset(&s->maps, 0, sizeof s->maps);
     for (int l = 0; l < nl; ++l) {
