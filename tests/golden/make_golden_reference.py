@@ -1,7 +1,9 @@
 """Writes tests/golden/reference_outputs.npz FROM THE REFERENCE ITSELF (oracle/_ref: GSLAM's own SE3, layouts and Vocabulary,
 compiled from the reference headers): what tests/test_oracle_ba.py, test_oracle_posegraph.py and test_oracle_bow.py compare the
 oracle against where oracle/_ref is not built.  Exact outputs of the vocabulary are stored as digests (oracle.digest).
-Run:  GSLAM_REFERENCE=<GSLAM checkout> python tests/golden/make_golden_reference.py"""
+With --se3-log-edges it writes tests/golden/se3_log_edges.npz only: SE3::log at the logarithm's branch points
+(tests/pose_graphs.se3_log_edge_inputs), for test_oracle_posegraph.test_se3_log_branches_equal_the_reference_class.
+Run:  GSLAM_REFERENCE=<GSLAM checkout> python tests/golden/make_golden_reference.py [--se3-log-edges]"""
 import ctypes as C
 import os
 import sys
@@ -10,6 +12,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import oracle  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 from gslam_b200 import synth  # noqa: E402
@@ -105,5 +108,24 @@ def main():
     print(path, os.path.getsize(path), "bytes")
 
 
+def se3_log_edges():
+    import pose_graphs
+    oracle.build()
+    assert oracle.have_ref(), "oracle/_ref is not built: set GSLAM_REFERENCE to a GSLAM checkout"
+    R = oracle.ref()
+    T = pose_graphs.se3_log_edge_inputs()
+    LOG = np.zeros((T.shape[0], 6))
+    for k in range(T.shape[0]):
+        t = np.ascontiguousarray(T[k]); lg = np.zeros(6)
+        R.ref_se3_log(t.ctypes.data, lg.ctypes.data)
+        LOG[k] = lg
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "se3_log_edges.npz")
+    np.savez_compressed(path, pose=T, log=LOG)
+    print(path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
-    main()
+    if "--se3-log-edges" in sys.argv:
+        se3_log_edges()
+    else:
+        main()

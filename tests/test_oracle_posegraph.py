@@ -130,3 +130,57 @@ def test_mixed_graph_solves_and_respects_fixed_frames():
     bad = synth.synth_pose_edges(pb, seed=1); bad.se3_second[0] = pb.n_cams
     with pytest.raises(Exception):
         O.ba_solve(pb.copy(), bad, max_iterations=1)
+
+
+def test_se3_log_branches_equal_the_reference_class():
+    """The logarithm's branch points (tests/pose_graphs.se3_log_edge_inputs: the identity as +-q, n < 1e-10, exactly pi with w = +0
+    and -0, w = +-5e-11 inside the |w| < 1e-10 branch and +-2e-10 just outside, pi - 1e-6, -q of 0.5 / 1 / 3 rad) against the
+    reference's SE3::log: live where oracle/_ref is built (which must still give the stored values), else as stored from it in
+    tests/golden/se3_log_edges.npz.  The sign of the rotation at pi follows the reference's w > 0 test (w = -0 gives -pi)."""
+    import pose_graphs
+    G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "se3_log_edges.npz"))
+    T, want = G["pose"], G["log"]
+    assert np.array_equal(T, pose_graphs.se3_log_edge_inputs())
+    if oracle.have_ref():
+        R = O.ref()
+        for t, w in zip(T, want):
+            t = np.ascontiguousarray(t); live = np.zeros(6)
+            R.ref_se3_log(t.ctypes.data, live.ctypes.data)
+            assert np.array_equal(live, w)
+    for t, w in zip(T, want):
+        got = O.se3_log(t)
+        assert np.abs(got - w).max() <= 1e-15 * max(1.0, np.abs(w).max()), (t, got, w)
+        # the rotation part is the shortest one: |w| <= pi, and for w < 0 it points against the quaternion's axis
+        assert np.linalg.norm(got[3:]) <= np.pi * (1 + 1e-15)
+        if t[3] < 0 and np.linalg.norm(t[:3]) > 0:
+            assert np.dot(got[3:], t[:3]) < 0
+
+
+# relative error of the pose-graph gradient (through the Bernoulli series of J_l^-1 truncated after ad^8) against central
+# differences of the cost, one GPS edge with identity information and residual [v = (1, 0.5, -0.3), w = angle * axis]; measured
+# (DESIGN.md section 2).  At 0.5 rad the series is exact to the central differences' own error (~1e-10).
+SERIES_ERROR = {0.5: None, 1.0: 4.9e-8, 2.0: 1.63e-5, 2.5: 1.32e-4, 3.0: 7.3e-4}
+
+
+@pytest.mark.parametrize("angle", list(SERIES_ERROR))
+def test_truncated_jl_inv_series_error_is_as_recorded(angle):
+    import pose_graphs
+    axis = pose_graphs._unit(np.array([0.3, -0.5, 0.8]))
+    E = np.concatenate([pose_graphs._residual_quat(angle, axis), [1.0, 0.5, -0.3]])
+    pb = pose_graphs._pose_graph(np.array([[0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0]]))
+    pe = pose_graphs._edges(gps=[0], gmeas=synth.se3_inv(E)[None], ginfo=np.eye(6)[None])
+    assert abs(np.linalg.norm(O.se3_log(O.se3_mul(E, np.r_[0, 0, 0, 1.0, 0, 0, 0]))[3:]) - angle) < 1e-12
+    g = O.ba_linearize(pb, 0.0, pe)["gc"][0]
+    h = 1e-5
+    num = np.zeros(6)
+    for a in range(6):
+        d = np.zeros((1, 6)); d[0, a] = h
+        plus = pb.copy(); plus.cam_pose_wc = retract_wc(pb.cam_pose_wc, d)
+        minus = pb.copy(); minus.cam_pose_wc = retract_wc(pb.cam_pose_wc, -d)
+        num[a] = (O.ba_cost(plus, 0.0, pe) - O.ba_cost(minus, 0.0, pe)) / (2 * h)
+    err = np.abs(-num - g).max() / np.abs(num).max()
+    want = SERIES_ERROR[angle]
+    if want is None:
+        assert err < 1e-9, err
+    else:   # the truncation itself, not the differences' noise: pinned within a factor 1.5 either way
+        assert want / 1.5 < err < want * 1.5, err
