@@ -302,7 +302,13 @@ int gb_match_stereo(gb_ctx* ctx, const gb_keypoint* kps_left, const uint8_t* des
 int gb_match_download(gb_ctx* ctx, gb_features* fq, int32_t* best_idx, int32_t* best_dist, int32_t* second_dist, int* n) {
   if (!ctx || !fq || !n) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  if (fq->n_matched < 0) GB_CHECK(gb_features_count(ctx, fq, &fq->n_matched));  // (the match was enqueued behind an extraction in flight)
+  if (fq->n_matched < 0) {  // (the match was enqueued behind an extraction in flight)
+    // resolved only when the extraction succeeded: after a failed one every call fails the same way, instead of the second
+    // reporting the count the failure left behind (0 matches, or more rows than the feature set holds)
+    int nq = 0;
+    GB_CHECK(gb_features_count(ctx, fq, &nq));
+    fq->n_matched = nq;
+  }
   const int cap = *n, cnt = fq->n_matched;
   *n = cnt;
   if (cnt > cap) {

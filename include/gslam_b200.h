@@ -103,9 +103,11 @@ typedef struct gb_orb_cfg {
   int32_t fast_threshold; /* 20                                         */
 } gb_orb_cfg;
 #define GB_ORB_MAX_LEVELS 12
-/* A pyramid level keeps at most 4096 keypoints (its selection sorts in shared memory); a configuration whose per-level quota plus ties
- * exceeds that -- nfeatures beyond ~15 000 at the default 8 levels -- fails with GB_ERR_CAPACITY instead of truncating (cv::ORB has no
- * such limit; the SLAM configurations of BASELINE.json use 1000 / 2000). */
+/* A pyramid level keeps at most 4096 keypoints (its selection sorts in shared memory): the level's quota plus the keypoints tied with
+ * the last one kept (equal Harris response) must be <= 4096, or the extraction fails with GB_ERR_CAPACITY instead of truncating
+ * (cv::ORB has no such limit; the SLAM configurations of BASELINE.json use 1000 / 2000).  Level 0 has the largest quota: at the
+ * default scale 1.2 and 8 levels it is 4096 at nfeatures = 18 862 and 4097 at 18 863, so frames without such ties extract up to
+ * nfeatures = 18 862. */
 GB_API void gb_orb_cfg_default(gb_orb_cfg* cfg);
 
 /*

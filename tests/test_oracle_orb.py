@@ -206,3 +206,25 @@ def test_gray_conversion_equals_cv2():
     assert np.array_equal(oracle.to_gray(img3, rgb=True), cv2.cvtColor(img3, cv2.COLOR_RGB2GRAY))
     assert np.array_equal(oracle.to_gray(img4), cv2.cvtColor(img4, cv2.COLOR_BGRA2GRAY))
     assert np.array_equal(oracle.to_gray(img4, rgb=True), cv2.cvtColor(img4, cv2.COLOR_RGBA2GRAY))
+
+
+from _orb_limits import CASES as LIMIT_CASES, OVER_CAP, check_reach, level0_fast_corners  # noqa: E402
+
+
+@pytest.mark.parametrize("case", LIMIT_CASES + [OVER_CAP], ids=lambda c: c.id)
+def test_limit_case_oracle_equals_cv2(case):
+    """The ORB limit cases (edge thresholds 22..239, 12 levels, scale factors 1.01..3.7, FAST thresholds 1 and 254, the 4096-keypoint
+    level cap and one past it, 16384-pixel sides): the oracle reaches each case's boundary and equals live cv2 in every keypoint field
+    and descriptor bit, so the device parity tests of tests/test_orb_limits_gpu.py compare against cv2's answer."""
+    img = case.image()
+    kps, desc = oracle.orb_extract(img, case.nfeatures, **case.kw)
+    check_reach(case, kps, fast0=level0_fast_corners(case, img))
+    pytest.importorskip("cv2")
+    import sys
+    sys.path.insert(0, GD)
+    from make_golden_orb import cv2_orb_canonical
+    want, wdesc, _ = cv2_orb_canonical(img, case.nfeatures, **case.cv2_kw)
+    assert len(kps) == len(want)
+    for f in ("octave", "x", "y", "size", "angle", "response"):
+        assert np.array_equal(kps[f], want[f]), f
+    assert np.array_equal(desc, wdesc)
