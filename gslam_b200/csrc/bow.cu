@@ -259,9 +259,12 @@ int gb_voc_destroy(gb_ctx* ctx, gb_vocabulary* v) {
   return GB_OK;
 }
 
-static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, const int* d_count, int levelsup, uint64_t* words, float* values,
+// pending (nullable): the feature set of an extraction in flight whose rows d_feats are -- the walk is clipped by its device-side
+// count, and its status word comes back with the results: a failed extraction fails the call instead of reading as an empty frame.
+static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, gb_features* pending, int levelsup, uint64_t* words, float* values,
                    int* n_words, uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
   if (n == 0) { *n_words = 0; *n_fv = 0; return GB_OK; }
+  const int* d_count = pending ? pending->d_count : nullptr;
   const int npad = next_pow2(n);
   const bool in_smem = npad <= kSmemKeys;
   GB_CHECK(gb_dev_realloc(ctx, (void**)&v->d_fword, &v->fword_cap, (size_t)n * 12));
@@ -278,10 +281,17 @@ static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, c
       n, d_count, npad, v->weighting, v->scoring, f_word, f_node, f_weight, in_smem ? nullptr : v->d_keys, (int*)v->d_out,
       (unsigned long long*)(v->d_out + o_words), (float*)(v->d_out + o_val), (unsigned long long*)(v->d_out + o_node), (uint32_t*)(v->d_out + o_feat));
   GB_LAUNCH_CHECK(ctx);
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bytes + 1024));
+  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bytes + 2048));
   uint8_t* h = (uint8_t*)gb_stage_alloc(ctx, bytes);
+  int* hc = pending ? (int*)gb_stage_alloc(ctx, 2 * sizeof(int)) : nullptr;
   GB_CUDA(ctx, cudaMemcpyAsync(h, v->d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  if (hc) GB_CUDA(ctx, cudaMemcpyAsync(hc, d_count, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (hc) {
+    int cnt = 0;
+    const int rc = gb_features_resolve(ctx, pending, hc, &cnt);
+    if (rc != GB_OK) { *n_words = 0; *n_fv = 0; return rc; }
+  }
   const int nw = ((int*)h)[0], m = ((int*)h)[1];
   *n_words = nw; *n_fv = m;
   memcpy(words, h + o_words, (size_t)nw * 8);
@@ -310,7 +320,7 @@ int gb_bow_transform_features(gb_ctx* ctx, gb_vocabulary* v, gb_features* f, int
   CtxLock lk(ctx);
   // the descriptors of an extraction still in flight: the launch is sized for the capacity and clipped by the device-side count
   const int n = f->h_count >= 0 ? f->h_count : f->capacity;
-  return bow_run(ctx, v, (const uint4*)f->d_desc, n, f->h_count >= 0 ? nullptr : f->d_count, levelsup, words, values, n_words, fv_node, fv_feat, n_fv);
+  return bow_run(ctx, v, (const uint4*)f->d_desc, n, f->h_count >= 0 ? nullptr : f, levelsup, words, values, n_words, fv_node, fv_feat, n_fv);
 }
 
 }  // extern "C"

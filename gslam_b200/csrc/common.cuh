@@ -53,6 +53,7 @@ struct gb_features {
   uint8_t* d_desc = nullptr;     // [capacity*32], 32-byte rows
   int* d_count = nullptr;        // device-side keypoint count (written by extract)
   int* d_status = nullptr;       // device-side status word (0 ok, else required capacity)
+  int* d_train_status = nullptr; // status word of the train set of the last match with this set as query (written by the match)
   int h_count = -1;              // host copy (valid when >=0)
   int expect = 0;                // expected row count while h_count is unknown (nfeatures of the extraction in flight): tunes launches
   int32_t* d_best = nullptr;     // match outputs [capacity]
@@ -62,6 +63,10 @@ struct gb_features {
 };
 
 void gb_set_error(gb_ctx* ctx, const char* fmt, ...);
+// The {count, status} pair an extraction left in f->d_count, read back to the host as hc: on success sets f->h_count and *n to the
+// count; else returns GB_ERR_CAPACITY with the reason in the error text and *n = the capacity the extraction needed (0: an
+// internal overflow).
+int gb_features_resolve(gb_ctx* ctx, gb_features* f, const int* hc, int* n);
 // A ctx on `device` that enqueues on `stream`, which another ctx owns and must outlive it (gb_ctx_destroy leaves it alone).
 int gb_ctx_create_on_stream(int device, cudaStream_t stream, gb_ctx** out);
 int gb_stage_reserve(gb_ctx* ctx, size_t bytes);           // make sure the pinned staging holds >= bytes

@@ -251,17 +251,18 @@ int gb_features_create(gb_ctx* ctx, int capacity, gb_features** out) {
   size_t cap = (size_t)capacity;
   cudaError_t e = cudaMalloc((void**)&f->d_kps, cap * sizeof(gb_keypoint));
   if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_desc, cap * 32);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_count, 2 * sizeof(int));
+  if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_count, 4 * sizeof(int));  // count, status, train status, (pad)
   if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_best, cap * sizeof(int32_t));
   if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_dist, cap * sizeof(int32_t));
   if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_dist2, cap * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMemsetAsync(f->d_count, 0, 2 * sizeof(int), ctx->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(f->d_count, 0, 4 * sizeof(int), ctx->stream);
   if (e != cudaSuccess) {
     gb_set_error(ctx, "gb_features_create(%d) -> %s", capacity, cudaGetErrorString(e));
     gb_features_destroy(ctx, f);
     return GB_ERR_CUDA;
   }
   f->d_status = f->d_count + 1;
+  f->d_train_status = f->d_count + 2;
   f->h_count = 0;
   *out = f;
   return GB_OK;
@@ -283,6 +284,25 @@ int gb_features_destroy(gb_ctx* ctx, gb_features* f) {
   return GB_OK;
 }
 
+}  // extern "C"
+
+int gb_features_resolve(gb_ctx* ctx, gb_features* f, const int* hc, int* n) {
+  if (hc[1] < 0) {
+    *n = 0;
+    gb_set_error(ctx, "extract: internal overflow (%s)", hc[1] == -2 ? "more than 4096 keypoints kept on one level" : "candidate buffer");
+    return GB_ERR_CAPACITY;
+  }
+  if (hc[1] != 0) {
+    *n = hc[1];
+    gb_set_error(ctx, "extract kept %d keypoints but the feature set holds %d", hc[1], f->capacity);
+    return GB_ERR_CAPACITY;
+  }
+  f->h_count = *n = hc[0];
+  return GB_OK;
+}
+
+extern "C" {
+
 int gb_features_count(gb_ctx* ctx, gb_features* f, int* n) {
   if (!ctx || !f || !n) return GB_ERR_INVALID;
   CtxLock lk(ctx);
@@ -290,19 +310,25 @@ int gb_features_count(gb_ctx* ctx, gb_features* f, int* n) {
     int hc[2] = {0, 0};
     GB_CUDA(ctx, cudaMemcpyAsync(hc, f->d_count, sizeof hc, cudaMemcpyDeviceToHost, ctx->stream));
     GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (hc[1] < 0) {
-      *n = 0;
-      gb_set_error(ctx, "extract: internal overflow (%s)", hc[1] == -2 ? "more than 4096 keypoints kept on one level" : "candidate buffer");
-      return GB_ERR_CAPACITY;
-    }
-    if (hc[1] != 0) {
-      *n = hc[1];
-      gb_set_error(ctx, "extract kept %d keypoints but the feature set holds %d", hc[1], f->capacity);
-      return GB_ERR_CAPACITY;
-    }
-    f->h_count = hc[0];
+    return gb_features_resolve(ctx, f, hc, n);
   }
   *n = f->h_count;
+  return GB_OK;
+}
+
+// test hook: put a feature set back into the state of an extraction in flight -- device-side {count, status} as given, host count
+// unknown, `expect` as the launch hint -- so that the device-count paths run on chosen rows (uploaded before)
+GB_API int gb_dbg_features_set_pending(gb_ctx* ctx, gb_features* f, int count, int status, int expect) {
+  if (!ctx || !f || count < 0 || count > f->capacity) return GB_ERR_INVALID;
+  CtxLock lk(ctx);
+  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + 1024));
+  int* hc = (int*)gb_stage_alloc(ctx, 2 * sizeof(int));
+  hc[0] = count;
+  hc[1] = status;
+  GB_CUDA(ctx, cudaMemcpyAsync(f->d_count, hc, 2 * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  f->h_count = -1;
+  f->expect = expect;
   return GB_OK;
 }
 
@@ -366,18 +392,8 @@ int gb_features_download(gb_ctx* ctx, gb_features* f, gb_keypoint* kps, uint8_t*
   if (hd && rows > 0) GB_CUDA(ctx, cudaMemcpyAsync(hd, f->d_desc, (size_t)rows * 32, cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (speculative) {
-    if (hc[1] < 0) {
-      *n = 0;
-      gb_set_error(ctx, "extract: internal overflow (%s)", hc[1] == -2 ? "more than 4096 keypoints kept on one level" : "candidate buffer");
-      return GB_ERR_CAPACITY;
-    }
-    if (hc[1] != 0) {
-      *n = hc[1];
-      gb_set_error(ctx, "extract kept %d keypoints but the feature set holds %d", hc[1], f->capacity);
-      return GB_ERR_CAPACITY;
-    }
-    f->h_count = cnt = hc[0];
-    *n = cnt;
+    GB_CHECK(gb_features_resolve(ctx, f, hc, n));
+    cnt = *n;
     if (cnt > cap) {
       gb_set_error(ctx, "gb_features_download: %d keypoints > caller capacity %d", cnt, cap);
       return GB_ERR_CAPACITY;

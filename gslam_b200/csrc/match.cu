@@ -26,6 +26,8 @@ __device__ __forceinline__ int ham256(const uint4& a0, const uint4& a1, const ui
 
 // d_nq / d_nt (nullable): device-side row counts of an extraction still in flight -- the launch is then sized for the capacities
 // passed as nq / nt and the kernel clips to the real counts, so that extract -> match chains without a host round trip.
+// train_status (nullable): receives the train set's status word (d_nt[1], the word after a gb_features count; 0 when the train
+// count is on the host), so that the download of the query set can tell a failed train extraction from an empty train set.
 // STEREO (rectified pair, left = query, right = train): a right keypoint is a candidate of a left one iff
 // |y_R - y_L| <= band and min_disp <= x_L - x_R <= max_disp (level-0 pixel coordinates, float compares); everything else -- the
 // distance, the (distance, index) order, the tie rule -- is the matcher's.  The right keypoints' (x, y) ride along with the staged
@@ -41,9 +43,11 @@ __global__ void __launch_bounds__(kQPerCta) match_kernel(const uint4* __restrict
                                                          int nt, int chunk, MatchPartial* __restrict__ partial,
                                                          unsigned int* __restrict__ tickets, int32_t* __restrict__ best_idx,
                                                          int32_t* __restrict__ best_dist, int32_t* __restrict__ second_dist,
-                                                         const int* __restrict__ d_nq, const int* __restrict__ d_nt, StereoArgs st) {
+                                                         const int* __restrict__ d_nq, const int* __restrict__ d_nt,
+                                                         int* __restrict__ train_status, StereoArgs st) {
   gb_pdl_launch_dependents();
   gb_pdl_wait();
+  if (train_status && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *train_status = d_nt ? d_nt[1] : 0;
   const int pstride = nq;  // layout of the partials: [split][query capacity]
   if (d_nq) nq = min(max(*d_nq, 0), nq);
   if (d_nt) nt = min(max(*d_nt, 0), nt);
@@ -165,6 +169,7 @@ struct MatchState {
   size_t partial_cap = 0;
   void* d_tickets = nullptr;
   size_t tickets_cap = 0;
+  int last_plan[4] = {0, 0, 0, 0};  // qtiles, nsplit, chunk, stereo of the last launch (gb_dbg_match_last_plan); 0s: none launched
 };
 
 void gb_match_state_free(gb_ctx* ctx) {
@@ -177,13 +182,20 @@ void gb_match_state_free(gb_ctx* ctx) {
 
 // Enqueue the match of (d_q, nq) against (d_t, nt) on the ctx stream.  Outputs are device pointers (may be null).
 // nq / nt: row counts, or -- with d_nq / d_nt -- CAPACITIES the launch must cover while the real counts are read on the device; the
-// work split is then tuned for the expected counts eq / et (<= 0: unknown, use the capacities).
+// work split is then tuned for the expected counts eq / et (<= 0: unknown, use the capacities).  d_train_status: see match_kernel.
 int gb_match_launch(gb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, int nt, int32_t* d_best, int32_t* d_dist,
                     int32_t* d_dist2, const int* d_nq = nullptr, const int* d_nt = nullptr, const StereoArgs* stereo = nullptr, int eq = 0,
-                    int et = 0) {
-  if (nq <= 0) return GB_OK;
+                    int et = 0, int* d_train_status = nullptr) {
   if (!ctx->match) ctx->match = new MatchState();
   MatchState* ms = ctx->match;
+  if (nq <= 0) {  // no query rows: nothing to launch, but the download still has to see the train set's status
+    ms->last_plan[0] = ms->last_plan[1] = ms->last_plan[2] = 0;
+    ms->last_plan[3] = stereo != nullptr;
+    if (d_train_status)
+      GB_CUDA(ctx, d_nt ? cudaMemcpyAsync(d_train_status, d_nt + 1, sizeof(int), cudaMemcpyDeviceToDevice, ctx->stream)
+                        : cudaMemsetAsync(d_train_status, 0, sizeof(int), ctx->stream));
+    return GB_OK;
+  }
   const int qtiles = gb_div_up(nq, kQPerCta);
   if (eq <= 0 || eq > nq) eq = nq;
   if (et <= 0 || et > nt) et = nt;
@@ -211,12 +223,16 @@ int gb_match_launch(gb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t,
   const size_t smem = (size_t)chunk * (stereo ? 40 : 32);
   StereoArgs sa = {};
   if (stereo) sa = *stereo;
+  ms->last_plan[0] = qtiles;
+  ms->last_plan[1] = nsplit;
+  ms->last_plan[2] = chunk;
+  ms->last_plan[3] = stereo != nullptr;
   if (stereo)
     GB_CUDA(ctx, gb_launch_pdl(match_kernel<true>, grid, dim3(kQPerCta), smem, ctx->stream, (const uint4*)d_q, nq, (const uint4*)d_t, nt > 0 ? nt : 0, chunk,
-                               (MatchPartial*)ms->d_partial, (unsigned int*)ms->d_tickets, d_best, d_dist, d_dist2, d_nq, d_nt, sa));
+                               (MatchPartial*)ms->d_partial, (unsigned int*)ms->d_tickets, d_best, d_dist, d_dist2, d_nq, d_nt, d_train_status, sa));
   else
     GB_CUDA(ctx, gb_launch_pdl(match_kernel<false>, grid, dim3(kQPerCta), smem, ctx->stream, (const uint4*)d_q, nq, (const uint4*)d_t, nt > 0 ? nt : 0, chunk,
-                               (MatchPartial*)ms->d_partial, (unsigned int*)ms->d_tickets, d_best, d_dist, d_dist2, d_nq, d_nt, sa));
+                               (MatchPartial*)ms->d_partial, (unsigned int*)ms->d_tickets, d_best, d_dist, d_dist2, d_nq, d_nt, d_train_status, sa));
   GB_LAUNCH_CHECK(ctx);
   return GB_OK;
 }
@@ -250,6 +266,14 @@ GB_API int gb_dbg_popc_peak(gb_ctx* ctx, double* popc_per_s) {
   return GB_OK;
 }
 
+// test hook: the work split of the last match launch on this ctx -- {query tiles, train splits, rows per split, stereo}
+GB_API int gb_dbg_match_last_plan(gb_ctx* ctx, int* out) {
+  if (!ctx || !out) return GB_ERR_INVALID;
+  CtxLock lk(ctx);
+  for (int i = 0; i < 4; ++i) out[i] = ctx->match ? ctx->match->last_plan[i] : 0;
+  return GB_OK;
+}
+
 int gb_match_features(gb_ctx* ctx, gb_features* fq, gb_features* ft) {
   if (!ctx || !fq || !ft) return GB_ERR_INVALID;
   CtxLock lk(ctx);
@@ -258,7 +282,7 @@ int gb_match_features(gb_ctx* ctx, gb_features* fq, gb_features* ft) {
     fq->n_matched = -1;  // resolved by gb_match_download
     return gb_match_launch(ctx, fq->d_desc, fq->h_count >= 0 ? fq->h_count : fq->capacity, ft->d_desc, ft->h_count >= 0 ? ft->h_count : ft->capacity,
                            fq->d_best, fq->d_dist, fq->d_dist2, fq->h_count >= 0 ? nullptr : fq->d_count, ft->h_count >= 0 ? nullptr : ft->d_count,
-                           nullptr, fq->expect, ft->expect);
+                           nullptr, fq->expect, ft->expect, fq->d_train_status);
   }
   const int nq = fq->h_count, nt = ft->h_count;
   fq->n_matched = nq;
@@ -275,7 +299,8 @@ int gb_match_stereo_features(gb_ctx* ctx, gb_features* left, gb_features* right,
   left->n_matched = async ? -1 : left->h_count;
   return gb_match_launch(ctx, left->d_desc, left->h_count >= 0 ? left->h_count : left->capacity, right->d_desc,
                          right->h_count >= 0 ? right->h_count : right->capacity, left->d_best, left->d_dist, left->d_dist2,
-                         left->h_count >= 0 ? nullptr : left->d_count, right->h_count >= 0 ? nullptr : right->d_count, &sa, left->expect, right->expect);
+                         left->h_count >= 0 ? nullptr : left->d_count, right->h_count >= 0 ? nullptr : right->d_count, &sa, left->expect, right->expect,
+                         async ? left->d_train_status : nullptr);
 }
 
 // Host-buffer variant (what the Svar module's match_stereo binds).
@@ -303,10 +328,25 @@ int gb_match_download(gb_ctx* ctx, gb_features* fq, int32_t* best_idx, int32_t* 
   if (!ctx || !fq || !n) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   if (fq->n_matched < 0) {  // (the match was enqueued behind an extraction in flight)
-    // resolved only when the extraction succeeded: after a failed one every call fails the same way, instead of the second
-    // reporting the count the failure left behind (0 matches, or more rows than the feature set holds)
-    int nq = 0;
-    GB_CHECK(gb_features_count(ctx, fq, &nq));
+    // resolved only when both extractions succeeded: the query set's {count, status} and the train set's status, which the match
+    // copied next to them, come back in one synchronisation.  After a failed extraction every call fails the same way, instead of
+    // the second reporting the count the failure left behind (0 matches, or more rows than the feature set holds), and instead of
+    // a failed train set reading as an empty one (-1 / 257 / 257 for every query).
+    GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + 1024));
+    int* hs = (int*)gb_stage_alloc(ctx, 4 * sizeof(int));
+    GB_CUDA(ctx, cudaMemcpyAsync(hs, fq->d_count, 3 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    int nq = fq->h_count;
+    if (nq < 0) GB_CHECK(gb_features_resolve(ctx, fq, hs, &nq));
+    if (hs[2] < 0) {
+      gb_set_error(ctx, "gb_match_download: the extraction of the train set failed (internal overflow: %s)",
+                   hs[2] == -2 ? "more than 4096 keypoints kept on one level" : "candidate buffer");
+      return GB_ERR_CAPACITY;
+    }
+    if (hs[2] != 0) {
+      gb_set_error(ctx, "gb_match_download: the extraction of the train set kept %d keypoints, more than its feature set holds", hs[2]);
+      return GB_ERR_CAPACITY;
+    }
     fq->n_matched = nq;
   }
   const int cap = *n, cnt = fq->n_matched;

@@ -148,7 +148,12 @@ GB_API int gb_features_download(gb_ctx* ctx, gb_features* f, gb_keypoint* kps, u
  */
 GB_API int gb_match_hamming(gb_ctx* ctx, const uint8_t* query, int nq, const uint8_t* train, int nt, int32_t* best_idx,
                             int32_t* best_dist, int32_t* second_dist);
-/* Device-resident: match fq against ft; results stay on device until gb_match_download. */
+/* Device-resident: match fq against ft; results stay on device until gb_match_download.  Either set may be the output of an
+ * extraction still in flight (gb_orb_extract_to): the match is then enqueued behind it and reads the row counts on the device.
+ * gb_match_download: on input *n is the capacity of the (nullable) output arrays, on output the number of queries matched; when
+ * that is more than the capacity it returns GB_ERR_CAPACITY and writes none of the arrays.  If the extraction of fq OR of ft
+ * failed (more keypoints kept than the feature set holds, or an internal overflow) it returns GB_ERR_CAPACITY naming the failed
+ * side, on every call, rather than matches against an empty set. */
 GB_API int gb_match_features(gb_ctx* ctx, gb_features* fq, gb_features* ft);
 GB_API int gb_match_download(gb_ctx* ctx, gb_features* fq, int32_t* best_idx, int32_t* best_dist, int32_t* second_dist,
                              int* n);
@@ -159,7 +164,8 @@ GB_API int gb_match_download(gb_ctx* ctx, gb_features* fq, int32_t* best_idx, in
  * min_disparity <= x_L - x_R <= max_disparity (float compares on GSLAM::KeyPoint::pt, level-0 pixels, Map.h:180-194); among the
  * candidates the same distance (hamming32, Vocabulary.h:485-491), (distance, index) order and tie rule as gb_match_hamming.
  * best_idx = -1 / distances 257 when a left keypoint has no candidate.  The reference has no stereo matcher: this definition is
- * ours (DESIGN.md).  Device-resident variant: results stay with `left` until gb_match_download(left).
+ * ours (DESIGN.md).  band_rows < 0 or NaN, or max_disparity < min_disparity: GB_ERR_INVALID.  Device-resident variant: results stay
+ * with `left` until gb_match_download(left), which fails as above when the extraction of `left` or of `right` failed.
  */
 GB_API int gb_match_stereo(gb_ctx* ctx, const gb_keypoint* kps_left, const uint8_t* desc_left, int n_left,
                            const gb_keypoint* kps_right, const uint8_t* desc_right, int n_right, float band_rows,
@@ -192,7 +198,9 @@ GB_API int gb_remap_apply(gb_ctx* ctx, gb_remap* map, const uint8_t* src, int ch
  * floats (accumulated and normalised with the same operations).  A leaf above level L - levelsup files under itself (the reference
  * reads an uninitialised node id there).  gb_bow_transform_features: the same for descriptors already resident in HBM (the output
  * of gb_orb_extract_to), no host round trip before the walk; the output arrays must hold the CAPACITY of `f` entries (the row
- * count of an extraction still in flight is only known on the device; the launch is clipped by it). */
+ * count of an extraction still in flight is only known on the device; the launch is clipped by it).  If that extraction failed
+ * (more keypoints kept than `f` holds, or an internal overflow) it returns GB_ERR_CAPACITY with *n_words = *n_fv = 0, on every
+ * call, rather than an empty BowVector. */
 typedef struct gb_vocabulary gb_vocabulary;
 GB_API int gb_voc_create(gb_ctx* ctx, int k, int L, int weighting, int scoring, uint32_t n_nodes, const uint32_t* child_num, const float* weight,
                          const uint8_t* desc32, gb_vocabulary** out);

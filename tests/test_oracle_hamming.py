@@ -8,6 +8,8 @@ import pytest
 import oracle
 from gslam_b200 import synth
 
+import _match_cases as MC
+
 G = np.load(os.path.join(os.path.dirname(__file__), "golden", "hamming_golden.npz"))
 
 
@@ -77,25 +79,7 @@ def test_edge_cases():
     assert idx.size == 0
 
 
-def _stereo_numpy(kl, dl, kr, dr, band, mind, maxd):
-    """Independent restatement of the stereo row-band rule (vectorised numpy, stable argsort on (distance, index))."""
-    nl = len(kl)
-    idx = np.full(nl, -1, np.int32); d1 = np.full(nl, 257, np.int32); d2 = np.full(nl, 257, np.int32)
-    if len(kr) == 0:
-        return idx, d1, d2
-    bits_r = np.unpackbits(dr, axis=1)
-    for i in range(nl):
-        dy = np.abs(kr["y"] - kl["y"][i]).astype(np.float32)
-        disp = (kl["x"][i] - kr["x"]).astype(np.float32)
-        cand = np.nonzero((dy <= np.float32(band)) & (disp >= np.float32(mind)) & (disp <= np.float32(maxd)))[0]
-        if cand.size == 0:
-            continue
-        d = (np.unpackbits(dl[i])[None, :] != bits_r[cand]).sum(axis=1)
-        order = np.lexsort((cand, d))
-        idx[i] = cand[order[0]]; d1[i] = d[order[0]]
-        if cand.size > 1:
-            d2[i] = d[order[1]]
-    return idx, d1, d2
+_stereo_numpy = MC.stereo_numpy
 
 
 def _stereo_case(rng, nl, nr, dup=False):
@@ -121,3 +105,57 @@ def test_stereo_rowband_match_equals_numpy_restatement():
     kl, dl, kr, dr = _stereo_case(rng, 100, 120)
     a = oracle.match_stereo(kl, dl, kr, dr, 1e9, -1e9, 1e9); b = oracle.match_hamming(dl, dr)
     assert all(np.array_equal(x, y) for x, y in zip(a, b))
+
+
+# ---- the matcher's work split and the stereo predicate at their edges (tests/_match_cases.py; the device side is
+# tests/test_match_paths_gpu.py) ----------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("sm", MC.SM_COUNTS)
+@pytest.mark.parametrize("case", MC.CASES, ids=lambda c: c.id)
+def test_match_case_reaches_its_boundary(case, sm):
+    MC.check_reach(case, case.plan(sm), sm)
+
+
+def test_match_plan_mirror_known_splits():
+    """The planner's splits for the shapes of the parity tests and beyond them, at 132 SMs."""
+    want = {(2000, 2000): (16, 17, 120), (513, 4097): (5, 52, 80), (3000, 50): (24, 2, 32), (40000, 5000): (313, 5, 1024),
+            (1, 100000): (1, 261, 384), (33665, 100): (264, 1, 104), (33536, 100): (262, 2, 56), (10, 0): (1, 1, 8), (0, 10): (0, 0, 0)}
+    for (nq, nt), p in want.items():
+        assert MC.plan(nq, nt, sm_count=132) == p, (nq, nt)
+    # the expect hints of a count still on the device: below the launch size they shape the split, above it they are ignored
+    assert MC.plan(4256, 4256, 2039, 2039) == (34, 36, 120)
+    assert MC.plan(4256, 4256, 9999, 9999) == MC.plan(4256, 4256) == MC.plan(4256, 4256, 0, 0)
+    for sm in MC.SM_COUNTS:  # every split but the last is full, and the splits cover the train rows
+        for nq, nt, eq, et in [(1, 1, 0, 0), (7, 33, 0, 0), (300, 2000, 0, 500), (5000, 70000, 100, 0), (1, 8193, 0, 256)]:
+            qt, ns, ch = MC.plan(nq, nt, eq, et, sm)
+            assert qt * MC.KQ >= nq and (ns - 1) * ch < nt <= ns * ch and ch % 8 == 0 and ch <= MC.MAX_CHUNK
+
+
+@pytest.mark.parametrize("case", [c for c in MC.CASES if c.stereo is not None], ids=lambda c: c.id)
+def test_stereo_case_oracle_equals_numpy(case):
+    s = case.shape(132); d = case.data(132)
+    kl, kr = d["kl"][:s.nq], d["kr"][:s.nt]
+    got = oracle.match_stereo(kl, d["q"][:s.nq], kr, d["t"][:s.nt], *case.stereo)
+    want = _stereo_numpy(kl, d["q"][:s.nq], kr, d["t"][:s.nt], *case.stereo)
+    for g, w in zip(got, want):
+        assert np.array_equal(g, w)
+    assert (got[0] >= 0).sum() > s.nq // 2 if s.nt else (got[0] == -1).all()
+
+
+@pytest.mark.parametrize("edge", MC.STEREO_EDGES, ids=lambda e: e.id)
+def test_stereo_edge_oracle_equals_numpy(edge):
+    """The oracle's stereo predicate against the numpy restatement exactly where it is decided: |dy| == band (band 0 too),
+    disparities on min_disp and max_disp (min == max, negative windows), infinite windows and bands, -0.0, float disparities that
+    round near 16384, NaN coordinates."""
+    kl, dl, kr, dr, band, mind, maxd = edge.make(np.random.default_rng(5))
+    MC.stereo_hits(edge, kl, kr, band, mind, maxd)
+    got = oracle.match_stereo(kl, dl, kr, dr, band, mind, maxd)
+    want = _stereo_numpy(kl, dl, kr, dr, band, mind, maxd)
+    for g, w in zip(got, want):
+        assert np.array_equal(g, w)
+    if "nan" in edge.hits:  # a NaN coordinate is never a candidate, whatever the band and window
+        assert (got[0][np.isnan(kl["x"]) | np.isnan(kl["y"])] == -1).all()
+        bad = np.isnan(kr["x"]) | np.isnan(kr["y"])
+        assert not np.isin(got[0], np.nonzero(bad)[0]).any()
+        assert (got[0][~(np.isnan(kl["x"]) | np.isnan(kl["y"]))] >= 0).all()
+    if edge.id == "one_candidate":
+        assert (got[0][:-1] == np.arange(len(kl) - 1)).all() and (got[2] == 257).all() and got[0][-1] == -1 and got[1][-1] == 257
