@@ -151,6 +151,7 @@ _DEBUG_SIGNATURES = [
     ("gb_dbg_popc_peak", C.c_int, [_VP, C.POINTER(C.c_double)]),
     ("gb_dbg_match_last_plan", C.c_int, [_VP, _VP]),
     ("gb_dbg_features_set_pending", C.c_int, [_VP, _VP, C.c_int, C.c_int, C.c_int]),
+    ("gb_dbg_bow_last_plan", C.c_int, [_VP, _VP]),
     ("gb_dbg_orb_level_size", C.c_int, [C.c_int, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("gb_dbg_orb_candidates", C.c_int, [_VP, C.c_int, _VP, _VP, _VP, _VP, C.c_int, C.POINTER(C.c_int), _VP, C.c_int, C.POINTER(C.c_int)]),
 ]

@@ -12,9 +12,15 @@
 //            run heads -> the BowVector in std::map order, values accumulated exactly as the reference does (float, += the word's
 //            weight once per occurrence in feature order; first occurrence only for IDF / BINARY), L1 / L2 norm in double over the
 //            words in ascending order, FeatureVector flattened in map order.
-// Integer outputs (words, nodes, feature indices) are bit-exact; values are bit-exact unless the double norm needs more than 53 bits
-// (the norm is folded in a fixed tree, the reference adds sequentially: both are exact for float weights spanning < 2^29).
+// Integer outputs (words, nodes, feature indices) and values are bit-exact.  The norm's terms (|v| or v*v as floats) are all
+// multiples of 2^q for the smallest exponent q of their lowest set bits; while their sum stays below 2^(q+53) every partial sum is a
+// double, so any order of summation gives the same norm.  The kernel folds the norm in a fixed tree (thread chunks, warps, the
+// block); when that total is not below 2^(q+52) (one bit of margin for the tree's own rounding) one thread adds the terms again in
+// ascending word order, as the reference does.  L1 norms of idf-like weights stay far inside the bound; L2 norms of weights that
+// span many octaves (squares keep 24 significant bits over twice the span) can leave it, and then the sequential sum runs.
 // A leaf met above level L - levelsup leaves the reference's node id uninitialised (:1579,1728); it files under the leaf itself here.
+// One vocabulary may be used from any ctx on its device, from any thread: its per-call scratch is guarded by its own lock, held
+// until the call's stream is synchronised.
 #include "common.cuh"
 
 struct gb_vocabulary {
@@ -23,11 +29,13 @@ struct gb_vocabulary {
   uint32_t* d_child = nullptr;  // [n_nodes]
   float* d_weight = nullptr;    // [n_nodes]
   uint4* d_desc = nullptr;      // [n_nodes][2]
+  std::mutex mu;                // guards everything below across a whole transform (the callers' ctxs may differ)
   // per-call scratch (grow-only): per-feature word / node / weight, sorted keys (large inputs), outputs
   uint8_t* d_feat = nullptr; size_t feat_cap = 0;
   uint32_t* d_fword = nullptr; size_t fword_cap = 0;  // [n] word, [n] node, [n] weight bits
   unsigned long long* d_keys = nullptr; size_t keys_cap = 0;  // [2][npad] when the keys do not fit shared memory
   uint8_t* d_out = nullptr; size_t out_cap = 0;       // [counts(4 ints) | words u64[n] | fv_node u64[n] | values f32[n] | fv_feat u32[n]]
+  int last_plan[5] = {0, 0, 0, 0, 0};  // of the last launch (gb_dbg_bow_last_plan): G, keys in smem, npad launched, npad sorted, flags
 };
 
 namespace {
@@ -131,7 +139,17 @@ __device__ __forceinline__ double block_sum_d(double v, double* s_part) {
   return s_part[32];
 }
 
-// out_counts: [0] words, [1] feature-vector entries
+constexpr int kNoTerm = 1 << 20;  // lsb exponent of a zero term: exact in any order, bounds nothing
+
+// t >= 0 (a norm term): the exponent q of its lowest set bit, t = odd * 2^q
+__device__ __forceinline__ int lsb_exponent(float t) {
+  const unsigned b = __float_as_uint(t), e = b >> 23, m = b & 0x7fffffu;
+  if (b == 0u) return kNoTerm;
+  return (e ? (int)e - 150 : -149) + __ffs(e ? (m | 0x800000u) : m) - 1;
+}
+
+// out_counts: [0] words, [1] feature-vector entries, [2] keys sorted (npad after a device-side count), [3] flags: 1 = the node
+// keys were not sorted (every live word is its own node), 2 = the norm was re-summed sequentially
 __global__ void __launch_bounds__(kRedThreads, 1) bow_reduce_kernel(int n, const int* __restrict__ d_count, int npad, int weighting, int scoring,
                                                                     const uint32_t* __restrict__ f_word, const uint32_t* __restrict__ f_node,
                                                                     const float* __restrict__ f_weight, unsigned long long* __restrict__ gkeys,
@@ -141,7 +159,8 @@ __global__ void __launch_bounds__(kRedThreads, 1) bow_reduce_kernel(int n, const
   extern __shared__ __align__(16) unsigned long long s_keys[];
   __shared__ int s_warp[32];
   __shared__ double s_part[33];
-  __shared__ int s_same;
+  __shared__ int s_same, s_qmin;
+  __shared__ double s_seq;
   unsigned long long* kw = gkeys ? gkeys : s_keys;  // word keys
   unsigned long long* kn = kw + npad;               // node keys (npad = the allocated power of two, sized for the capacity)
   if (d_count) {  // descriptors of an extraction in flight: the launch was sized for the capacity, sort only what the count needs
@@ -150,7 +169,7 @@ __global__ void __launch_bounds__(kRedThreads, 1) bow_reduce_kernel(int n, const
     while (p2 < n) p2 <<= 1;
     npad = min(npad, p2);
   }
-  if (threadIdx.x == 0) s_same = 1;
+  if (threadIdx.x == 0) { s_same = 1; s_qmin = kNoTerm; }
   __syncthreads();
   int differ = 0;
   for (int i = threadIdx.x; i < npad; i += kRedThreads) {
@@ -180,6 +199,7 @@ __global__ void __launch_bounds__(kRedThreads, 1) bow_reduce_kernel(int n, const
   (void)block_exscan(live, s_warp, &m);
   const bool tf = weighting == W_TF || weighting == W_TF_IDF;
   double local = 0.0;  // this thread's share of the norm, its words in ascending order
+  int qmin = kNoTerm;  // the smallest lsb exponent of its terms
   for (int i = i0; i < i1; ++i) {
     const unsigned long long key = kw[i];
     if (key == ~0ull) break;
@@ -190,13 +210,28 @@ __global__ void __launch_bounds__(kRedThreads, 1) bow_reduce_kernel(int n, const
         for (int t = i + 1; t < npad && (kw[t] >> 32) == (key >> 32); ++t) v = __fadd_rn(v, w);  // += per occurrence (:357-369)
       words[pos] = key >> 32;
       values[pos] = v;
-      local += scoring == S_L2 ? (double)__fmul_rn(v, v) : (double)fabsf(v);
+      const float term = scoring == S_L2 ? __fmul_rn(v, v) : fabsf(v);
+      local += (double)term;
+      qmin = min(qmin, lsb_exponent(term));
       ++pos;
     }
   }
+  qmin = __reduce_min_sync(0xffffffffu, qmin);
+  if ((threadIdx.x & 31) == 0) atomicMin(&s_qmin, qmin);  // (read after the barriers of block_sum_d)
   const bool must = scoring != S_DOT;
+  bool sequential = false;
   if (must || (tf && nw > 0)) {
     double norm = block_sum_d(local, s_part);  // (values of other threads are visible after its barriers)
+    if (must && !(norm < ldexp(1.0, s_qmin + 52))) {  // the tree may have rounded differently: the reference's order (:382-408)
+      sequential = true;                               // (block-uniform: every thread read the same norm and s_qmin)
+      if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int a = 0; a < nw; ++a) s += scoring == S_L2 ? (double)__fmul_rn(values[a], values[a]) : (double)fabsf(values[a]);
+        s_seq = s;
+      }
+      __syncthreads();
+      norm = s_seq;
+    }
     if (must && scoring == S_L2) norm = sqrt(norm);
     if (!must) norm = (double)nw;                // TF / TF_IDF without normalisation: divided by the number of words (:1592-1598)
     if (norm > 0.0)
@@ -208,7 +243,7 @@ __global__ void __launch_bounds__(kRedThreads, 1) bow_reduce_kernel(int n, const
     fv_node[i] = src[i] >> 32;
     fv_feat[i] = (uint32_t)src[i];
   }
-  if (threadIdx.x == 0) { out_counts[0] = nw; out_counts[1] = m; }
+  if (threadIdx.x == 0) { out_counts[0] = nw; out_counts[1] = m; out_counts[2] = npad; out_counts[3] = (same ? 1 : 0) | (sequential ? 2 : 0); }
 }
 
 int next_pow2(int n) { int p = 2; while (p < n) p <<= 1; return p; }
@@ -263,6 +298,7 @@ int gb_voc_destroy(gb_ctx* ctx, gb_vocabulary* v) {
 // count, and its status word comes back with the results: a failed extraction fails the call instead of reading as an empty frame.
 static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, gb_features* pending, int levelsup, uint64_t* words, float* values,
                    int* n_words, uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
+  for (int& x : v->last_plan) x = 0;
   if (n == 0) { *n_words = 0; *n_fv = 0; return GB_OK; }
   const int* d_count = pending ? pending->d_count : nullptr;
   const int npad = next_pow2(n);
@@ -287,6 +323,7 @@ static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, g
   GB_CUDA(ctx, cudaMemcpyAsync(h, v->d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   if (hc) GB_CUDA(ctx, cudaMemcpyAsync(hc, d_count, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  v->last_plan[0] = G; v->last_plan[1] = in_smem; v->last_plan[2] = npad; v->last_plan[3] = ((int*)h)[2]; v->last_plan[4] = ((int*)h)[3];
   if (hc) {
     int cnt = 0;
     const int rc = gb_features_resolve(ctx, pending, hc, &cnt);
@@ -301,11 +338,8 @@ static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, g
   return GB_OK;
 }
 
-int gb_bow_transform(gb_ctx* ctx, gb_vocabulary* v, const uint8_t* desc, int n, int levelsup, uint64_t* words, float* values, int* n_words,
-                     uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
-  if (!ctx || !v || n < 0 || (n > 0 && !desc) || !words || !values || !n_words || !fv_node || !fv_feat || !n_fv) return GB_ERR_INVALID;
-  CtxLock lk(ctx);
-  if (n == 0) { *n_words = 0; *n_fv = 0; return GB_OK; }
+static int bow_upload_run(gb_ctx* ctx, gb_vocabulary* v, const uint8_t* desc, int n, int levelsup, uint64_t* words, float* values,
+                          int* n_words, uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
   GB_CHECK(gb_dev_realloc(ctx, (void**)&v->d_feat, &v->feat_cap, (size_t)n * 32));
   GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + (size_t)n * 32 + 1024));
   uint8_t* h = (uint8_t*)gb_stage_alloc(ctx, (size_t)n * 32);
@@ -314,13 +348,39 @@ int gb_bow_transform(gb_ctx* ctx, gb_vocabulary* v, const uint8_t* desc, int n, 
   return bow_run(ctx, v, (const uint4*)v->d_feat, n, nullptr, levelsup, words, values, n_words, fv_node, fv_feat, n_fv);
 }
 
+// A call that failed half way may leave work on the scratch in flight: it must end before the vocabulary's lock is released.
+static int bow_finish(gb_ctx* ctx, int rc) {
+  if (rc != GB_OK) cudaStreamSynchronize(ctx->stream);
+  return rc;
+}
+
+int gb_bow_transform(gb_ctx* ctx, gb_vocabulary* v, const uint8_t* desc, int n, int levelsup, uint64_t* words, float* values, int* n_words,
+                     uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
+  if (!ctx || !v || n < 0 || (n > 0 && !desc) || !words || !values || !n_words || !fv_node || !fv_feat || !n_fv) return GB_ERR_INVALID;
+  CtxLock lk(ctx);
+  std::lock_guard<std::mutex> vl(v->mu);
+  if (n == 0) { for (int& x : v->last_plan) x = 0; *n_words = 0; *n_fv = 0; return GB_OK; }
+  return bow_finish(ctx, bow_upload_run(ctx, v, desc, n, levelsup, words, values, n_words, fv_node, fv_feat, n_fv));
+}
+
 int gb_bow_transform_features(gb_ctx* ctx, gb_vocabulary* v, gb_features* f, int levelsup, uint64_t* words, float* values, int* n_words,
                               uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
   if (!ctx || !v || !f || !words || !values || !n_words || !fv_node || !fv_feat || !n_fv) return GB_ERR_INVALID;
   CtxLock lk(ctx);
+  std::lock_guard<std::mutex> vl(v->mu);
   // the descriptors of an extraction still in flight: the launch is sized for the capacity and clipped by the device-side count
   const int n = f->h_count >= 0 ? f->h_count : f->capacity;
-  return bow_run(ctx, v, (const uint4*)f->d_desc, n, f->h_count >= 0 ? nullptr : f, levelsup, words, values, n_words, fv_node, fv_feat, n_fv);
+  return bow_finish(ctx, bow_run(ctx, v, (const uint4*)f->d_desc, n, f->h_count >= 0 ? nullptr : f, levelsup, words, values, n_words, fv_node,
+                                 fv_feat, n_fv));
+}
+
+// test hook: the plan of the last transform with this vocabulary -- {lanes per descriptor, keys in shared memory, keys launched,
+// keys sorted, flags (1: node keys not sorted, 2: norm re-summed in word order)}; 0s: nothing launched
+GB_API int gb_dbg_bow_last_plan(gb_vocabulary* v, int* out) {
+  if (!v || !out) return GB_ERR_INVALID;
+  std::lock_guard<std::mutex> vl(v->mu);
+  for (int i = 0; i < 5; ++i) out[i] = v->last_plan[i];
+  return GB_OK;
 }
 
 }  // extern "C"

@@ -195,7 +195,9 @@ GB_API int gb_remap_apply(gb_ctx* ctx, gb_remap* map, const uint8_t* src, int ch
  * Map.h:321), host memory.  Outputs, caller-owned, capacity n each: the BowVector (std::map<WordId,float>, :47) as parallel arrays
  * in map order (words ascending) and the FeatureVector (std::map<NodeId,std::vector<unsigned>>, :48) flattened in map order (node
  * ascending, feature indices ascending).  Word / node / feature indices are bit-exact with the reference; values are the reference's
- * floats (accumulated and normalised with the same operations).  A leaf above level L - levelsup files under itself (the reference
+ * floats, bit-exact for every vocabulary (accumulated with the same operations; the double L1 / L2 norm equals the reference's
+ * sum in ascending word order).  One vocabulary may be used from any ctx on the device it was created on, from any thread: calls
+ * on it are serialised by the vocabulary itself.  A leaf above level L - levelsup files under itself (the reference
  * reads an uninitialised node id there).  gb_bow_transform_features: the same for descriptors already resident in HBM (the output
  * of gb_orb_extract_to), no host round trip before the walk; the output arrays must hold the CAPACITY of `f` entries (the row
  * count of an extraction still in flight is only known on the device; the launch is clipped by it).  If that extraction failed

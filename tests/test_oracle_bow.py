@@ -150,3 +150,71 @@ def test_empty_and_single_inputs():
     assert all(e[k].size == 0 for k in KEYS)
     one = O.bow_transform(v, z["q_a"][:1], 0)
     assert one["words"].size == 1 and one["values"][0] == np.float32(1.0) and one["fv_feat"].tolist() == [0]
+
+
+# ---- the cases of tests/_bow_cases.py: boundaries of the device's launch plan, and the norm's order of summation ------------------
+import _bow_cases as BC  # noqa: E402
+
+
+@pytest.mark.parametrize("case", BC.CASES, ids=lambda c: c.id)
+def test_case_reaches_its_boundary(case):
+    """The mirror of the launch plan reaches the boundary each case was written for, and the mirror of the reduce kernel's
+    BowVector (words, run sums, norm fold with its exactness predicate) gives the oracle's words and values."""
+    BC.check_reach(case)
+    v, f, lu = case.data
+    ref = O.bow_transform(v, f, lu)
+    fold = BC.norm_fold(v, ref)
+    assert np.array_equal(fold["words"], ref["words"])
+    assert np.array_equal(BC.mirror_values(v, fold), ref["values"])
+
+
+def test_tree_norm_differs_from_the_reference_on_the_adversarial_case():
+    """IDF / L1 over 65 538 words (1, w, and 65 536 x 2^-54): the norm folded in the kernel's tree keeps 2^-38 that the reference's
+    sequential sum absorbs, and the second word's value comes out one float apart -- unless the sequential re-sum runs."""
+    v, f, lu = BC.BY_ID["norm_adversarial"].data
+    ref = O.bow_transform(v, f, lu)
+    fold = BC.norm_fold(v, ref)
+    assert fold["tree"] != fold["seq"] and fold["q"] == -54 and BC.sequential_needed(fold)
+    tree = BC.normalise(v, fold, fold["tree"])
+    diff = np.nonzero(tree != ref["values"])[0]
+    assert diff.tolist() == [1] and ref["values"][1] == np.float32(0.26592186) and tree[1] == np.float32(0.26592183)
+    assert np.array_equal(BC.normalise(v, fold, fold["seq"]), ref["values"])
+
+
+@pytest.mark.parametrize("cid", ["norm_inside_l1", "norm_inside_l2", "norm_l1_bench_like", "norm_l2_bench_like", "norm_l1_wide_idf"])
+def test_tree_norm_equals_the_reference_inside_the_bound(cid):
+    v, f, lu = BC.BY_ID[cid].data
+    ref = O.bow_transform(v, f, lu)
+    fold = BC.norm_fold(v, ref)
+    assert not BC.sequential_needed(fold)
+    assert fold["tree"] == fold["seq"] and np.array_equal(BC.normalise(v, fold, fold["tree"]), ref["values"])
+
+
+def test_plan_mirror_at_device_counts():
+    """npad is launched for the capacity and clipped to the count's power of two (at least 2) on the device."""
+    assert BC.plan(10, 3000, 0) == (16, 1, 4096, 2, 1)
+    assert BC.plan(10, 3000, 1) == (16, 1, 4096, 2, 1)
+    assert BC.plan(20, 3000, 1234) == (32, 1, 4096, 2048, 2)
+    assert BC.plan(10, 12000, 8192) == (16, 0, 16384, 8192, 8)
+    assert BC.plan(10, 12000, 8193) == (16, 0, 16384, 16384, 16)
+    assert BC.plan(10, 12000, 12000) == (16, 0, 16384, 16384, 16)
+    assert BC.plan(17, 1, None) == (32, 1, 2, 2, 1) and BC.plan(16, 0, None) == (0, 0, 0, 0, 0)
+
+
+@pytest.mark.parametrize("case", BC.CASES, ids=lambda c: c.id)
+def test_case_oracle_equals_live_reference(case):
+    """Where oracle/_ref is built: the oracle equals Vocabulary::transform on every case the reference defines (not a negative
+    levelsup, no walk ending above level L - levelsup: the reference reads an uninitialised node id there)."""
+    if not oracle.have_ref():
+        pytest.skip("oracle/_ref not built")
+    if not BC.reference_defined(case):
+        pytest.skip("the reference leaves the node id undefined here")
+    v, f, lu = case.data
+    R = O.RefVocabulary.from_arrays(v)
+    try:
+        want = R.transform(f, lu)
+    finally:
+        R.close()
+    got = O.bow_transform(v, f, lu)
+    for k in KEYS:
+        assert np.array_equal(got[k], want[k], equal_nan=k == "values"), k
