@@ -1942,7 +1942,19 @@ int gb_ba_graph_begin(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt_in) 
     gb_set_error(ctx, "gb_ba: only PROJECTION_PINHOLE (Optimizer.h:59) is implemented");
     return GB_ERR_INVALID;
   }
-  if (opt.max_iterations < 0 || opt.pcg_max_iters < 0) return GB_ERR_INVALID;
+  if (opt.max_iterations < 0 || opt.pcg_max_iters < 0) {
+    gb_set_error(ctx, "gb_ba: max_iterations (%d) and pcg_max_iters (%d) must not be negative", opt.max_iterations, opt.pcg_max_iters);
+    return GB_ERR_INVALID;
+  }
+  // (a NaN lambda never leaves NaN and a zero one never leaves a reject streak; a NaN tolerance never stops)
+  if (!(std::isfinite(opt.lambda_init) && opt.lambda_init > 0.0)) {
+    gb_set_error(ctx, "gb_ba: lambda_init must be finite and > 0 (got %g)", opt.lambda_init);
+    return GB_ERR_INVALID;
+  }
+  if (std::isnan(opt.huber_delta) || std::isnan(opt.function_tolerance) || std::isnan(opt.pcg_tol)) {
+    gb_set_error(ctx, "gb_ba: huber_delta, function_tolerance and pcg_tol must not be NaN");
+    return GB_ERR_INVALID;
+  }
   if (opt.linear_solver != 0 && opt.linear_solver != 1) { gb_set_error(ctx, "gb_ba: linear_solver must be 0 (PCG) or 1 (direct)"); return GB_ERR_INVALID; }
   if (opt.linear_solver == 1 && g->d.npe > 0) { gb_set_error(ctx, "gb_ba: graphs with pose-graph terms use linear_solver = 0 (PCG)"); return GB_ERR_INVALID; }
   if (opt.linear_solver == 1 && g->d.nc > 0 && (!g->chol_ok || g->shard_world > 1)) {
@@ -2106,6 +2118,21 @@ int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
   return ba_compact_step(ctx, g, comm);
 }
 
+// The costs of a solve come from its LM decisions (lm_decide); one that made none still reports the cost at its input estimate as
+// both initial and final cost: a sweep, the pose-graph terms and the deterministic sum (all-reduced over the shards with a
+// communicator) into the LM scalars.
+int ba_cost_at_input(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
+  const BaDev& d = g->d;
+  cudaStream_t s = ctx->stream;
+  GB_CHECK(ba_launch_sweep(ctx, g, d, s, 3));
+  GB_CHECK(ba_pose_linearize(ctx, g, s));
+  ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np + d.npe), kRedThreads, 0, s>>>(d, d.cost_pt, d.np + d.npe, g->d_cost); GB_LAUNCH_CHECK(ctx);
+  if (comm) GB_CHECK(gb_comm_allreduce_sum_f64(comm, g->d_cost, 1));
+  GB_CUDA(ctx, cudaMemcpyAsync(&d.sc->initial_cost, g->d_cost, sizeof(double), cudaMemcpyDeviceToDevice, s));
+  GB_CUDA(ctx, cudaMemcpyAsync(&d.sc->cost, g->d_cost, sizeof(double), cudaMemcpyDeviceToDevice, s));
+  return GB_OK;
+}
+
 extern "C" {
 
 // single-CTA block-sparse PCG, in the variant that fits the graph's active cameras and its longest block row of S (the
@@ -2181,12 +2208,24 @@ static int ba_fill_result(gb_ctx* ctx, const BaScalars& h, gb_ba_result* res) {
   return GB_OK;
 }
 
+}  // extern "C"
+
+int ba_graph_finish_impl(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm, gb_ba_result* res) {
+  BaScalars h;
+  GB_CHECK(ba_read_scalars(ctx, g, &h));
+  if (h.iterations == 0) {
+    GB_CHECK(ba_cost_at_input(ctx, g, comm));
+    GB_CHECK(ba_read_scalars(ctx, g, &h));
+  }
+  return ba_fill_result(ctx, h, res);
+}
+
+extern "C" {
+
 int gb_ba_graph_finish(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* res) {
   if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  BaScalars h;
-  GB_CHECK(ba_read_scalars(ctx, g, &h));
-  return ba_fill_result(ctx, h, res);
+  return ba_graph_finish_impl(ctx, g, nullptr, res);
 }
 
 // local-BA fast path (block-CSR Schur + single-CTA PCG): 4 launches per LM iteration, for graphs whose estimate fits the
@@ -2233,6 +2272,7 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
     }
   }
   if (local4) { ba_install_pending_kernel<<<1, 1024, 0, ctx->stream>>>(g->d); GB_LAUNCH_CHECK(ctx); }
+  if (g->opt.max_iterations == 0) GB_CHECK(ba_cost_at_input(ctx, g, nullptr));
   GB_CUDA(ctx, cudaEventRecord(ctx->eve, ctx->stream));
   BaDev& dd = g->d;
   const size_t bp = pose_out ? (size_t)dd.nc * 56 : 0, bx = pts_out ? (size_t)dd.np * 24 : 0;

@@ -193,11 +193,13 @@ __global__ void __launch_bounds__(kCholThreads, 1) ba_chol_kernel(BaDev g, doubl
     }
   }
   __syncthreads();
-  // ---- E. solution (zero step when the factorisation broke down: LM rejects it and raises lambda) + retraction of the cameras
-  const bool fail = s_fail != 0;
+  // ---- E. solution (the whole step is zero when the factorisation broke down or a substitution left a non-finite component: LM
+  //      rejects it and raises lambda) + retraction of the cameras
+  int bad = 0;
+  for (int d = tid; d < n6; d += kCholThreads) bad |= !isfinite(y[d]);
+  const bool fail = __syncthreads_or(s_fail != 0 || bad) != 0;
   for (int d = tid; d < n6; d += kCholThreads) {
-    double v = fail ? 0.0 : y[d];
-    if (!isfinite(v)) v = 0.0;
+    const double v = fail ? 0.0 : y[d];
     y[d] = v;
     g.x[d] = v;
   }

@@ -287,7 +287,7 @@ int gb_ba_shard_solve(gb_comm* c, gb_ba_graph* g, const gb_ba_options* opt, gb_b
     }
   }
   GB_CUDA(ctx, cudaEventRecord(ctx->eve, ctx->stream));
-  GB_CHECK(gb_ba_graph_finish(ctx, g, res));
+  GB_CHECK(ba_graph_finish_impl(ctx, g, c, res));
   if (res) GB_CUDA(ctx, cudaEventElapsedTime(&res->gpu_ms, ctx->evs, ctx->eve));
   return GB_OK;
 }

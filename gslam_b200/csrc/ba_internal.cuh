@@ -103,6 +103,10 @@ int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
 // ba_compact_step = PCG, back-substitution + candidate cost (+ its all-reduce), LM accept / reject
 int ba_compact_reduce(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
 int ba_compact_step(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
+// the cost at the current estimate into the LM scalars' initial and final cost (a solve that made no LM decision); `comm`: all-reduced
+int ba_cost_at_input(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
+// gb_ba_graph_finish, with the cost of a zero-iteration solve all-reduced over `comm` (every rank calls it) when non-null
+int ba_graph_finish_impl(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm, gb_ba_result* res);
 
 // ---- ba_pose.cu -------------------------------------------------------------------------------------------------------------
 // pose-graph terms (SE3Edge / GPSEdge, Optimizer.h:127-148) on the stepwise dense-layout solver path

@@ -260,7 +260,9 @@ typedef struct gb_pose_edges {
   const double* gps_info;
 } gb_pose_edges;
 
-/* GSLAM::OptimzeConfig (Optimizer.h:174-182) + the solver knobs the reference leaves to its (absent) Ceres plugin. */
+/* GSLAM::OptimzeConfig (Optimizer.h:174-182) + the solver knobs the reference leaves to its (absent) Ceres plugin.
+ * A solve rejects (GB_ERR_INVALID) negative integer knobs, a lambda_init that is not finite and > 0, and a NaN huber_delta,
+ * function_tolerance or pcg_tol.  max_iterations = 0 runs no LM iteration and reports the cost at the input estimate. */
 typedef struct gb_ba_options {
   int32_t projection;       /* 0 = PROJECTION_PINHOLE (only 0 supported)                               */
   double huber_delta;       /* projectErrorHuberThreshold, 0.01 (normalised units); <=0 disables Huber */

@@ -773,6 +773,10 @@ int orc_ba_solve_ex(gb_ba_problem* pb, const gb_pose_edges* pe, const gb_ba_opti
   gb_ba_options opt;
   if (opt_in) opt = *opt_in; else { opt.projection = 0; opt.huber_delta = 0.01; opt.max_iterations = 500; opt.verbose = 0; opt.function_tolerance = 1e-6; opt.lambda_init = 1e-4; opt.pcg_max_iters = 50; opt.pcg_tol = 1e-10; opt.linear_solver = 0; }
   if (validate(pb) || validate_edges(pb, pe) || opt.projection != 0) return GB_ERR_INVALID;
+  /* the option checks of gb_ba_graph_begin */
+  if (opt.max_iterations < 0 || opt.pcg_max_iters < 0 || !(isfinite(opt.lambda_init) && opt.lambda_init > 0.0) || isnan(opt.huber_delta) ||
+      isnan(opt.function_tolerance) || isnan(opt.pcg_tol))
+    return GB_ERR_INVALID;
   ba_state s;
   state_init_ex(&s, pb, pe, opt.huber_delta);
   int nc = s.nc, np = s.np, n6 = 6 * nc;
