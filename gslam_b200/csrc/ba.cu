@@ -1508,12 +1508,19 @@ void gb_ba_options_default(gb_ba_options* o) {
 
 int gb_ba_graph_destroy(gb_ctx* ctx, gb_ba_graph* g) {
   if (!g) return GB_OK;
-  if (ctx && (!g->from_arena || g->sw_alloc || g->d.prof)) {
+  if (ctx) {
     CtxLock lk(ctx);
-    cudaStreamSynchronize(ctx->stream);
+    if (g->waiting) {  // another thread's solve of g is waiting on g's pinned scalars and events
+      gb_set_error(ctx, "gb_ba_graph_destroy: a solve of this graph is still waiting for the device on another thread");
+      return GB_ERR_INVALID;
+    }
+    if (!g->from_arena || g->sw_alloc || g->d.prof) cudaStreamSynchronize(ctx->stream);
   }
   ba_sweep_plan_drop(g);
   cudaFree(g->d.prof);
+  if (g->h_sc) cudaFreeHost(g->h_sc);
+  for (cudaEvent_t ev : {g->ev_s, g->ev_e, g->ev_done})
+    if (ev) cudaEventDestroy(ev);
   if (g->from_arena) {
     if (ctx) ctx->ba_arena_busy = false;
   } else {
@@ -2241,7 +2248,20 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   if (!ctx || !g) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
-  GB_CUDA(ctx, cudaEventRecord(ctx->evs, ctx->stream));
+  // A device-resident solve (no host outputs, not nested in another call on this ctx) waits for the device WITHOUT the ctx lock,
+  // on the graph's own pinned scalars and events: a tracking thread can then order its next frame after its match on this ctx
+  // (gb_ctx_wait_for) while the mapping thread still waits for this solve, and the next solve finds that frame already handed over.
+  // A second solve of g that another thread starts during that wait (g->waiting) takes the locked wait, leaving g's scalars and
+  // events to the first.
+  const bool unlocked_wait = !pose_out && !pts_out && ctx->lock_depth == 1 && !g->waiting;
+  if (unlocked_wait) {
+    if (!g->h_sc) GB_CUDA(ctx, cudaMallocHost((void**)&g->h_sc, sizeof(BaScalars)));
+    if (!g->ev_s) GB_CUDA(ctx, cudaEventCreate(&g->ev_s));
+    if (!g->ev_e) GB_CUDA(ctx, cudaEventCreate(&g->ev_e));
+    if (!g->ev_done) GB_CUDA(ctx, cudaEventCreateWithFlags(&g->ev_done, cudaEventDisableTiming));
+  }
+  cudaEvent_t ev_s = unlocked_wait ? g->ev_s : ctx->evs, ev_e = unlocked_wait ? g->ev_e : ctx->eve;
+  GB_CUDA(ctx, cudaEventRecord(ev_s, ctx->stream));
   const bool poll = g->opt.function_tolerance > 0.0 || g->opt.verbose;
   const bool local4 = ba_takes_local4(g);
   for (int it = 0; it < g->opt.max_iterations; ++it) {
@@ -2273,11 +2293,11 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   }
   if (local4) { ba_install_pending_kernel<<<1, 1024, 0, ctx->stream>>>(g->d); GB_LAUNCH_CHECK(ctx); }
   if (g->opt.max_iterations == 0) GB_CHECK(ba_cost_at_input(ctx, g, nullptr));
-  GB_CUDA(ctx, cudaEventRecord(ctx->eve, ctx->stream));
+  GB_CUDA(ctx, cudaEventRecord(ev_e, ctx->stream));
   BaDev& dd = g->d;
   const size_t bp = pose_out ? (size_t)dd.nc * 56 : 0, bx = pts_out ? (size_t)dd.np * 24 : 0;
   GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bp + bx + sizeof(BaScalars) + 1024));
-  BaScalars* hs = (BaScalars*)gb_stage_alloc(ctx, sizeof(BaScalars));
+  BaScalars* hs = unlocked_wait ? g->h_sc : (BaScalars*)gb_stage_alloc(ctx, sizeof(BaScalars));
   double* hp = bp ? (double*)gb_stage_alloc(ctx, bp + 8) : nullptr;
   double* hx = bx ? (double*)gb_stage_alloc(ctx, bx + 8) : nullptr;
   GB_CUDA(ctx, cudaMemcpyAsync(hs, dd.sc, sizeof(BaScalars), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2287,8 +2307,20 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
     GB_CUDA(ctx, cudaMemcpyAsync(hp, g->pose_wc_out, bp, cudaMemcpyDeviceToHost, ctx->stream));
   }
   if (hx) GB_CUDA(ctx, cudaMemcpyAsync(hx, dd.pts, bx, cudaMemcpyDeviceToHost, ctx->stream));
-  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (res) GB_CUDA(ctx, cudaEventElapsedTime(&res->gpu_ms, ctx->evs, ctx->eve));
+  if (unlocked_wait) {
+    GB_CUDA(ctx, cudaEventRecord(g->ev_done, ctx->stream));
+    cudaError_t done;
+    g->waiting = true;
+    {
+      CtxUnlock ul(ctx);
+      done = cudaEventSynchronize(g->ev_done);
+    }
+    g->waiting = false;
+    GB_CUDA(ctx, done);
+  } else {
+    GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  }
+  if (res) GB_CUDA(ctx, cudaEventElapsedTime(&res->gpu_ms, ev_s, ev_e));
   GB_CHECK(ba_fill_result(ctx, *hs, res));
   if (hp) memcpy(pose_out, hp, bp);
   if (hx) memcpy(pts_out, hx, bx);

@@ -58,6 +58,12 @@ struct gb_ba_graph {
   std::vector<int> cam_perm_h;      // host copy of cam_perm (camera-sorted slot -> sorted slot): refresh of a cached graph
   double* pose_wc_in = nullptr;     // device: the uploaded T_wc poses (blob), source of ba_prepare_kernel
   bool begun = false;
+  // what a device-resident solve waits on without holding the ctx lock (made on its first call): the LM scalars' pinned host copy,
+  // the solve's timing events and its completion event; `waiting` (read and written under the ctx lock) is set while a solve waits
+  // unlocked on them, so that nothing else reuses or frees them meanwhile
+  BaScalars* h_sc = nullptr;
+  cudaEvent_t ev_s = nullptr, ev_e = nullptr, ev_done = nullptr;
+  bool waiting = false;
   // PCG dispatch: single-CTA block-sparse kernel, else one-cluster kernel (pcg_cluster = 8/16), else generic multi-kernel
   bool pcg_sparse = false;
   size_t pcg_sparse_smem = 0;

@@ -155,4 +155,22 @@ struct CtxLock {
   }
 };
 
+// Releases a ctx that the calling thread holds exactly once (one CtxLock) for the scope of a host wait on the device, so that other
+// threads can enqueue on it meanwhile (gb_ctx_wait_for from a tracking thread while the mapping thread waits for its solve).
+// Nothing of the ctx's pinned staging may be waited on or read across it: another thread's CtxLock restarts the bump allocation and
+// gb_stage_reserve may free and reallocate the staging, so a gb_stage_alloc pointer taken before the unlock is invalid after it.
+struct CtxUnlock {
+  gb_ctx* c;
+  explicit CtxUnlock(gb_ctx* ctx) : c(ctx) {
+    c->lock_depth--;
+    c->mu.unlock();
+  }
+  ~CtxUnlock() {
+    c->mu.lock();
+    if (c->lock_depth++ == 0) cudaSetDevice(c->device);
+  }
+  CtxUnlock(const CtxUnlock&) = delete;
+  CtxUnlock& operator=(const CtxUnlock&) = delete;
+};
+
 static inline int gb_div_up(int a, int b) { return (a + b - 1) / b; }

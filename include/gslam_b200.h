@@ -22,8 +22,10 @@
  * fails with GB_ERR_NODEVICE and every compute entry point fails loudly.
  *
  * Threading: a gb_ctx owns one CUDA stream, its device buffers and pinned staging; calls on one ctx are serialised by an
- * internal mutex (the reference documents no re-entrancy guarantee, SURVEY.md §8b).  Use one ctx per calling thread for
- * concurrency (e.g. tracking thread: extract/match/pnp; mapping thread: local BA).
+ * internal mutex (the reference documents no re-entrancy guarantee, SURVEY.md §8b).  One exception: while gb_ba_graph_solve
+ * waits for the device it releases that mutex, so another thread's calls on the ctx (gb_ctx_wait_for from a tracking thread)
+ * run meanwhile.  One gb_ba_graph must not be used from two threads at once.  Use one ctx per calling thread for concurrency
+ * (e.g. tracking thread: extract/match/pnp; mapping thread: local BA).
  */
 #ifndef GSLAM_B200_H_
 #define GSLAM_B200_H_
@@ -310,6 +312,8 @@ GB_API int gb_ba_graph_create(gb_ctx* ctx, const gb_ba_problem* problem, gb_ba_g
 GB_API int gb_ba_graph_create_ex(gb_ctx* ctx, const gb_ba_problem* problem, const gb_pose_edges* edges, gb_ba_graph** out);
 GB_API int gb_ba_graph_destroy(gb_ctx* ctx, gb_ba_graph* g);
 GB_API int gb_ba_graph_reset(gb_ctx* ctx, gb_ba_graph* g); /* restore the uploaded estimate (device-to-device) */
+/* Solve from the current estimate and wait for it.  The wait does not hold the ctx (see Threading above); a second solve of g
+ * that another thread starts meanwhile waits holding it, and gb_ba_graph_destroy(g) meanwhile fails with GB_ERR_INVALID. */
 GB_API int gb_ba_graph_solve(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt, gb_ba_result* result);
 GB_API int gb_ba_graph_download(gb_ctx* ctx, gb_ba_graph* g, double* cam_pose_wc, double* points);
 /* One fused residual + Jacobian sweep at the current estimate (K6: V, g_p, W, U, g_c, cost stay on the device) — the
