@@ -2,6 +2,7 @@
 
 Names and argument meaning follow the reference (the production host side is the C++ plugins under plugin/):
   Context.orb_extract(img, nfeatures)   ~ the Svar module function gslam.b200.orb_extract(GImage, cfg)
+  Context.orb_extract_undistorted(remap, img, nfeatures) ~ gslam.b200.orb_extract_undistorted(GImage, Camera in, Camera out, cfg)
   Context.match_hamming(q, t)           ~ gslam.b200.match_hamming(GImage q, GImage t)
   Optimizer.optimize(graph)             ~ GSLAM::Optimizer::optimize(BundleGraph&)        Optimizer.h:229
   Optimizer.optimizePnP(matches, pose)  ~ GSLAM::Optimizer::optimizePnP(...)              Optimizer.h:202-207
@@ -163,6 +164,25 @@ class Context:
             self._check(rc)
             return kps[:n.value].copy(), desc[:n.value].copy()
 
+    def orb_extract_undistorted(self, remap: "Remap", img: np.ndarray, nfeatures: int = 500, capacity: int | None = None, **cfg_kw):
+        """orb_extract of the frame `remap` makes of img ((H, W) gray or (H, W, 3) colour of the map's input size), undistorted and
+        converted to gray on the device: one upload, one synchronisation.  Keypoints are in pixels of the map's output."""
+        rgb = bool(cfg_kw.pop("rgb", False))
+        img = np.ascontiguousarray(img, dtype=np.uint8)
+        ch = remap._channels(img)
+        cfg = self.orb_cfg(nfeatures=nfeatures, **cfg_kw)
+        cap = capacity or (2 * nfeatures + 256)
+        while True:
+            kps = np.zeros(cap, dtype=KP_DTYPE)
+            desc = np.zeros((cap, 32), dtype=np.uint8)
+            n = C.c_int(cap)
+            rc = self._lib.gb_orb_extract_undistorted(self._h, remap._h, ptr(img), ch, 1 if rgb else 0, C.byref(cfg), ptr(kps), ptr(desc), C.byref(n))
+            if rc == capi.GB_ERR_CAPACITY and capacity is None and n.value > cap:
+                cap = n.value
+                continue
+            self._check(rc)
+            return kps[:n.value].copy(), desc[:n.value].copy()
+
     # ---- match -------------------------------------------------------------------------------------------------------
     def match_hamming(self, query: np.ndarray, train: np.ndarray):
         """Returns (best_idx, best_dist, second_dist) int32 arrays, cv::BFMatcher(NORM_HAMMING) tie rules."""
@@ -235,6 +255,27 @@ class Remap:
         out = np.zeros(self.shape_out + ((ch,) if img.ndim == 3 else ()), np.uint8)
         self.ctx._check(self.ctx._lib.gb_remap_apply(self.ctx._h, self._h, ptr(img), ch, ptr(out)))
         return out
+
+    def _channels(self, img: np.ndarray) -> int:
+        """Channel count of a host frame, which must have the map's input size (the C calls take no size: they read w_in x h_in)."""
+        if img.ndim not in (2, 3) or img.shape[:2] != self.shape_in:
+            raise GbError(capi.GB_ERR_INVALID, f"frame of shape {img.shape} handed to a remap whose input is {self.shape_in}")
+        return 1 if img.ndim == 2 else img.shape[2]
+
+    def apply_to(self, img, d_dst: int, dst_pitch: int, channels: int = 1, device_ptr: bool = False, pitch: int | None = None, ctx: Context | None = None):
+        """Undistort into device memory at d_dst (h_out rows, dst_pitch bytes apart), enqueued on the stream of `ctx` (default: the
+        map's own).  img: numpy host array ((H, W) or (H, W, 3), rows `pitch` bytes apart when given, then `channels` counts), or an
+        integer device pointer when device_ptr."""
+        c = ctx or self.ctx
+        if device_ptr:
+            p = C.c_void_p(int(img))
+        else:
+            if pitch is None:
+                img = np.ascontiguousarray(img, np.uint8)
+                channels = self._channels(img)
+            p = ptr(img)
+        c._check(c._lib.gb_remap_apply_to(c._h, self._h, p, 1 if device_ptr else 0, pitch or self.shape_in[1] * channels, channels,
+                                          C.c_void_p(int(d_dst)), dst_pitch))
 
     def close(self):
         if getattr(self, "_h", None) and getattr(self.ctx, "_h", None):
@@ -309,6 +350,22 @@ class Features:
         else:
             p = ptr(img)
         c._check(c._lib.gb_orb_extract_to(c._h, p, 1 if device_ptr else 0, width, height, pitch or width, C.byref(cfg), self._h))
+
+    def extract_undistorted(self, remap: "Remap", img, cfg: capi.OrbCfg, channels: int = 1, rgb: bool = False, device_ptr: bool = False,
+                            pitch: int | None = None):
+        """extract() of the frame `remap` makes of img, which has the map's input size: a numpy host array ((H, W) or (H, W, 3), rows
+        `pitch` bytes apart when given, then `channels` counts), or an integer device pointer when device_ptr.  Enqueued on this
+        set's ctx; with a device frame nothing is synchronised."""
+        c = self.ctx
+        if device_ptr:
+            p = C.c_void_p(int(img))
+        else:
+            if pitch is None:
+                img = np.ascontiguousarray(img, np.uint8)
+                channels = remap._channels(img)
+            p = ptr(img)
+        c._check(c._lib.gb_orb_extract_undistorted_to(c._h, remap._h, p, 1 if device_ptr else 0, pitch or remap.shape_in[1] * channels, channels,
+                                                      1 if rgb else 0, C.byref(cfg), self._h))
 
     def count(self) -> int:
         n = C.c_int()

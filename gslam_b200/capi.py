@@ -92,6 +92,9 @@ _SIGNATURES = [
     ("gb_remap_create", C.c_int, [_VP, C.c_int, C.c_int, C.c_int, C.c_int, _VP, _VP, _VP, C.POINTER(_VP)]),
     ("gb_remap_destroy", C.c_int, [_VP, _VP]),
     ("gb_remap_apply", C.c_int, [_VP, _VP, _VP, C.c_int, _VP]),
+    ("gb_remap_apply_to", C.c_int, [_VP, _VP, _VP, C.c_int, C.c_int, C.c_int, _VP, C.c_int]),
+    ("gb_orb_extract_undistorted_to", C.c_int, [_VP, _VP, _VP, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(OrbCfg), _VP]),
+    ("gb_orb_extract_undistorted", C.c_int, [_VP, _VP, _VP, C.c_int, C.c_int, C.POINTER(OrbCfg), _VP, _VP, C.POINTER(C.c_int)]),
     ("gb_voc_create", C.c_int, [_VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint32, _VP, _VP, _VP, C.POINTER(_VP)]),
     ("gb_voc_destroy", C.c_int, [_VP, _VP]),
     ("gb_bow_transform", C.c_int, [_VP, _VP, _VP, C.c_int, C.c_int, _VP, _VP, C.POINTER(C.c_int), _VP, _VP, C.POINTER(C.c_int)]),

@@ -73,6 +73,16 @@ int gb_stage_reserve(gb_ctx* ctx, size_t bytes);           // make sure the pinn
 void* gb_stage_alloc(gb_ctx* ctx, size_t bytes);           // bump-allocate from pinned staging (256-B aligned), or nullptr
 int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes);  // grow-only device buffer
 
+// ---- undistortion in front of the ORB extraction: what remap.cu and orb.cu need of each other --------------------------------------
+// A dense device copy of a frame (`height` rows of `row_bytes`): the frame itself when it is a device pointer with pitch == row_bytes,
+// else a copy in the grow-only frame buffer of the ctx's ORB state (cudaMemcpy2DAsync on the ctx stream; pinned host memory directly,
+// pageable host memory through the ctx's pinned staging).  The copy is valid until the next call that stages a frame on this ctx.
+int gb_orb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row_bytes, int height, int pitch, const uint8_t** d_frame);
+void gb_remap_geometry(const gb_remap* m, int* device, int* w_in, int* h_in, int* w_out, int* h_out);
+// Enqueue the remap of the dense device frame d_src (w_in x h_in, 1 or 3 channels) as a GRAY w_out x h_out image at d_dst; d_dst and
+// dst_pitch must be multiples of 4 and dst_pitch >= w_out rounded up to 4 (every word of a row is stored whole).  Reads the map only.
+int gb_remap_enqueue_level0(gb_ctx* ctx, const gb_remap* m, const uint8_t* d_src, int channels, int rgb_order, uint8_t* d_dst, int dst_pitch);
+
 // Function attributes are per-function, per-DEVICE state shared by every ctx on the device: gb_func_setup sets kernel `fn`'s
 // dynamic shared-memory limit to `smem` bytes (GB_SMEM_OPTIN_MAX: the device's opt-in maximum less the kernel's static shared
 // memory) and, when `nonportable_cluster` is given, permits cluster sizes above 8, reporting there whether that worked.  Each

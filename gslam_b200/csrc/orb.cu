@@ -704,14 +704,18 @@ static int orb_cfg_check(gb_ctx* ctx, const gb_orb_cfg* c) {
   return GB_OK;
 }
 
+static int orb_state_create(gb_ctx* ctx) {
+  if (ctx->orb) return GB_OK;
+  ctx->orb = new OrbState();
+  GB_CUDA(ctx, cudaMalloc((void**)&ctx->orb->d_pattern, 1024));
+  GB_CUDA(ctx, cudaMemcpyAsync(ctx->orb->d_pattern, kOrbPattern, 1024, cudaMemcpyHostToDevice, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return GB_OK;
+}
+
 // (Re)build the per-resolution state: level geometry, quotas, resize tables, buffers.
 static int orb_prepare(gb_ctx* ctx, int w, int h, const gb_orb_cfg* cfg) {
-  if (!ctx->orb) {
-    ctx->orb = new OrbState();
-    GB_CUDA(ctx, cudaMalloc((void**)&ctx->orb->d_pattern, 1024));
-    GB_CUDA(ctx, cudaMemcpyAsync(ctx->orb->d_pattern, kOrbPattern, 1024, cudaMemcpyHostToDevice, ctx->stream));
-    GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  }
+  GB_CHECK(orb_state_create(ctx));
   OrbState* s = ctx->orb;
   if (s->valid && s->w == w && s->h == h && memcmp(&s->cfg, cfg, sizeof *cfg) == 0) return GB_OK;
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -875,6 +879,43 @@ static int orb_launch(gb_ctx* ctx, gb_features* out) {
   return GB_OK;
 }
 
+// Copy a frame into the dense frame buffer of the ctx's ORB state (d_color): pinned caller memory goes straight over PCIe, pageable
+// memory is staged through the ctx's pinned buffer.
+static int orb_stage_copy(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row, int height, int pitch) {
+  OrbState* s = ctx->orb;
+  const size_t bytes = row * height;
+  GB_CHECK(gb_dev_realloc(ctx, &s->d_color, &s->color_cap, bytes));
+  if (img_is_device) {
+    GB_CUDA(ctx, cudaMemcpy2DAsync(s->d_color, row, img, pitch, row, height, cudaMemcpyDeviceToDevice, ctx->stream));
+    return GB_OK;
+  }
+  cudaPointerAttributes at;
+  const bool pinned = cudaPointerGetAttributes(&at, img) == cudaSuccess && at.type == cudaMemoryTypeHost;
+  cudaGetLastError();
+  const uint8_t* src = img;
+  size_t spitch = (size_t)pitch;
+  if (!pinned) {
+    GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bytes + 1024));
+    uint8_t* hs = (uint8_t*)gb_stage_alloc(ctx, bytes);
+    for (int y = 0; y < height; ++y) memcpy(hs + (size_t)y * row, img + (size_t)y * pitch, row);
+    src = hs;
+    spitch = row;
+  }
+  GB_CUDA(ctx, cudaMemcpy2DAsync(s->d_color, row, src, spitch, row, height, cudaMemcpyHostToDevice, ctx->stream));
+  return GB_OK;
+}
+
+int gb_orb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row_bytes, int height, int pitch, const uint8_t** d_frame) {
+  if (img_is_device && (size_t)pitch == row_bytes) {
+    *d_frame = img;
+    return GB_OK;
+  }
+  GB_CHECK(orb_state_create(ctx));
+  GB_CHECK(orb_stage_copy(ctx, img, img_is_device, row_bytes, height, pitch));
+  *d_frame = (const uint8_t*)ctx->orb->d_color;
+  return GB_OK;
+}
+
 extern "C" {
 
 void gb_orb_cfg_default(gb_orb_cfg* c) {
@@ -905,25 +946,7 @@ static int orb_extract_to_impl(gb_ctx* ctx, const uint8_t* img, int img_is_devic
   OrbState* s = ctx->orb;
   const LevelInfo& L0 = s->P.lv[0];
   if (channels != 1) {
-    const size_t row = (size_t)width * channels, bytes = row * height;
-    GB_CHECK(gb_dev_realloc(ctx, &s->d_color, &s->color_cap, bytes));
-    if (img_is_device) {
-      GB_CUDA(ctx, cudaMemcpy2DAsync(s->d_color, row, img, pitch, row, height, cudaMemcpyDeviceToDevice, ctx->stream));
-    } else {
-      cudaPointerAttributes at;
-      const bool pinned = cudaPointerGetAttributes(&at, img) == cudaSuccess && at.type == cudaMemoryTypeHost;
-      cudaGetLastError();
-      const uint8_t* src = img;
-      int spitch = pitch;
-      if (!pinned) {
-        GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bytes + 1024));
-        uint8_t* hs = (uint8_t*)gb_stage_alloc(ctx, bytes);
-        for (int y = 0; y < height; ++y) memcpy(hs + (size_t)y * row, img + (size_t)y * pitch, row);
-        src = hs;
-        spitch = (int)row;
-      }
-      GB_CUDA(ctx, cudaMemcpy2DAsync(s->d_color, row, src, spitch, row, height, cudaMemcpyHostToDevice, ctx->stream));
-    }
+    GB_CHECK(orb_stage_copy(ctx, img, img_is_device, (size_t)width * channels, height, pitch));
     orb_gray_kernel<<<dim3(gb_div_up(width, 256), height), 256, 0, ctx->stream>>>((const uint8_t*)s->d_color, width, height, channels, rgb_order,
                                                                                  s->d_pyr + L0.off, L0.pitch);
     GB_LAUNCH_CHECK(ctx);
@@ -955,21 +978,67 @@ int gb_orb_extract_to(gb_ctx* ctx, const uint8_t* img, int img_is_device, int wi
   return orb_extract_to_impl(ctx, img, img_is_device, width, height, pitch, cfg_in, out, true);
 }
 
-static int orb_extract_host(gb_ctx* ctx, const uint8_t* img, int width, int height, int channels, int rgb_order, const gb_orb_cfg* cfg_in, gb_keypoint* kps,
-                            uint8_t* desc, int* n);
+// The same with the frame undistorted on the way into level 0: the state is prepared for the map's OUTPUT size, the (dense) source
+// is remapped, and converted to gray when it has 3 channels, by one kernel that writes level 0; then the usual chain.
+static int orb_extract_undistorted_impl(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int img_is_device, int pitch, int channels, int rgb_order,
+                                        const gb_orb_cfg* cfg_in, gb_features* out, bool sync_after) {
+  if (!ctx || !map || !img || !out) return GB_ERR_INVALID;
+  CtxLock lk(ctx);
+  int device, w_in, h_in, w_out, h_out;
+  gb_remap_geometry(map, &device, &w_in, &h_in, &w_out, &h_out);
+  if (channels != 1 && channels != 3) {
+    gb_set_error(ctx, "gb_orb_extract_undistorted: %d channels (1 or 3 are supported; the reference's 4-channel remap writes 3-channel pixels)", channels);
+    return GB_ERR_INVALID;
+  }
+  if (device != ctx->device) {
+    gb_set_error(ctx, "gb_orb_extract_undistorted: the map was created on device %d, the ctx is on device %d", device, ctx->device);
+    return GB_ERR_INVALID;
+  }
+  if (pitch < w_in * channels) {
+    gb_set_error(ctx, "gb_orb_extract_undistorted: pitch %d is shorter than a row of the map's %dx%d input with %d channels", pitch, w_in, h_in, channels);
+    return GB_ERR_INVALID;
+  }
+  gb_orb_cfg cfg;
+  if (cfg_in) cfg = *cfg_in; else gb_orb_cfg_default(&cfg);
+  GB_CHECK(orb_cfg_check(ctx, &cfg));
+  GB_CHECK(orb_prepare(ctx, w_out, h_out, &cfg));
+  const uint8_t* d_frame = nullptr;
+  GB_CHECK(gb_orb_stage_frame(ctx, img, img_is_device, (size_t)w_in * channels, h_in, pitch, &d_frame));
+  OrbState* s = ctx->orb;
+  const LevelInfo& L0 = s->P.lv[0];
+  GB_CHECK(gb_remap_enqueue_level0(ctx, map, d_frame, channels, rgb_order, s->d_pyr + L0.off, L0.pitch));
+  GB_CHECK(orb_launch(ctx, out));
+  if (!img_is_device && sync_after) GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staging / caller buffer may be reused
+  return GB_OK;
+}
+
+int gb_orb_extract_undistorted_to(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int img_is_device, int pitch, int channels, int rgb_order,
+                                  const gb_orb_cfg* cfg_in, gb_features* out) {
+  return orb_extract_undistorted_impl(ctx, map, img, img_is_device, pitch, channels, rgb_order, cfg_in, out, true);
+}
+
+// map == nullptr: the frame is width x height; else it is the map's input and width / height are not read
+static int orb_extract_host(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int width, int height, int channels, int rgb_order, const gb_orb_cfg* cfg_in,
+                            gb_keypoint* kps, uint8_t* desc, int* n);
+
+int gb_orb_extract_undistorted(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int channels, int rgb_order, const gb_orb_cfg* cfg_in, gb_keypoint* kps,
+                               uint8_t* desc, int* n) {
+  if (!map) return GB_ERR_INVALID;
+  return orb_extract_host(ctx, map, img, 0, 0, channels, rgb_order, cfg_in, kps, desc, n);
+}
 
 int gb_orb_extract(gb_ctx* ctx, const uint8_t* img, int width, int height, const gb_orb_cfg* cfg_in, gb_keypoint* kps, uint8_t* desc,
                    int* n) {
-  return orb_extract_host(ctx, img, width, height, 1, 0, cfg_in, kps, desc, n);
+  return orb_extract_host(ctx, nullptr, img, width, height, 1, 0, cfg_in, kps, desc, n);
 }
 
 int gb_orb_extract_image(gb_ctx* ctx, const uint8_t* img, int width, int height, int channels, int rgb_order, const gb_orb_cfg* cfg_in, gb_keypoint* kps,
                          uint8_t* desc, int* n) {
-  return orb_extract_host(ctx, img, width, height, channels, rgb_order, cfg_in, kps, desc, n);
+  return orb_extract_host(ctx, nullptr, img, width, height, channels, rgb_order, cfg_in, kps, desc, n);
 }
 
-static int orb_extract_host(gb_ctx* ctx, const uint8_t* img, int width, int height, int channels, int rgb_order, const gb_orb_cfg* cfg_in, gb_keypoint* kps,
-                            uint8_t* desc, int* n) {
+static int orb_extract_host(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int width, int height, int channels, int rgb_order, const gb_orb_cfg* cfg_in,
+                            gb_keypoint* kps, uint8_t* desc, int* n) {
   if (!ctx || !img || !n || *n < 0) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   gb_orb_cfg cfg;
@@ -982,7 +1051,13 @@ static int orb_extract_host(gb_ctx* ctx, const uint8_t* img, int width, int heig
     GB_CHECK(gb_features_create(ctx, want_cap, &ctx->tmp_f));
   }
   gb_features* f = ctx->tmp_f;
-  GB_CHECK(orb_extract_to_impl(ctx, img, 0, width, height, width * channels, &cfg, f, *n <= 0, channels, rgb_order));
+  if (map) {
+    int device, w_in, h_in, w_out, h_out;
+    gb_remap_geometry(map, &device, &w_in, &h_in, &w_out, &h_out);
+    GB_CHECK(orb_extract_undistorted_impl(ctx, map, img, 0, w_in * channels, channels, rgb_order, &cfg, f, *n <= 0));
+  } else {
+    GB_CHECK(orb_extract_to_impl(ctx, img, 0, width, height, width * channels, &cfg, f, *n <= 0, channels, rgb_order));
+  }
   const int cap = *n;
   if (cap > 0) {  // one synchronisation: the count travels with the rows
     int m = cap;

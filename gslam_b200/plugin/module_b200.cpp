@@ -9,6 +9,8 @@
 //                                                                     (Map.h:287,311-312)
 //   svar["gslam"]["b200"]["match_stereo"]  (kps_left, desc_left, kps_right, desc_right, Svar cfg) -> {"rightIdx", "distance", "distance2"}
 //   svar["gslam"]["b200"]["undistort"]     (GImage, Camera in, Camera out) -> GImage : GSLAM::Undistorter::undistort (Undistorter.h:271-348)
+//   svar["gslam"]["b200"]["orb_extract_undistorted"] (GImage, Camera in, Camera out, Svar cfg) -> {"keypoints", "descriptors"} : undistort,
+//                                          gray conversion and orb_extract in one device-resident pass; keypoints in camera_out pixels
 //   svar["gslam"]["b200"]["vocabulary"]    (std::shared_ptr<Vocabulary>) -> std::shared_ptr<Vocabulary> : the same vocabulary with the
 //                                          batch transforms (Vocabulary.h:174,192: virtual) answered by the device; any code holding
 //                                          a GSLAM::Vocabulary* / VocabularyPtr keeps working unchanged
@@ -63,7 +65,32 @@ gb_orb_cfg cfgFrom(GSLAM::Svar cfg) {
   return c;
 }
 
-bool extract(const GSLAM::GImage& img, GSLAM::Svar cfg, std::vector<GSLAM::KeyPoint>& kps, GSLAM::GImage& desc) {
+// The remap table of a camera pair, resident in HBM: built by the reference's own prepareReMap (Undistorter.h:120-203; every camera
+// model stays the reference's).  The table of the last pair is kept; it lives as long as the process-wide context it was created on.
+// Held by its users for the length of their call: a change of camera pair destroys the previous table.
+struct RemapCache {
+  std::mutex mtx;
+  std::string key;
+  gb_remap* map = nullptr;
+  gb_remap* get(gb_ctx* ctx, const GSLAM::Camera& in, const GSLAM::Camera& out) {  // call with mtx held
+    const std::string k = in.info() + "|" + out.info();
+    if (key == k && map) return map;
+    if (map) gb_remap_destroy(ctx, map);
+    map = nullptr;
+    GSLAM::UndistorterImpl table(in, out);
+    if (!table.valid || gb_remap_create(ctx, in.width(), in.height(), out.width(), out.height(), table.remapIdx, table.remapCoef, table.remapX, &map) != GB_OK)
+      return nullptr;
+    key = k;
+    return map;
+  }
+};
+RemapCache& remaps() {
+  static RemapCache c;
+  return c;
+}
+
+// remap != nullptr: img is the input of that table; it is undistorted (and converted to gray) on the way into the extraction
+bool extract(const GSLAM::GImage& img, GSLAM::Svar cfg, std::vector<GSLAM::KeyPoint>& kps, GSLAM::GImage& desc, gb_remap* remap = nullptr) {
   // 8UC1 gray, or the 8UC3 / 8UC4 colour frames GSLAM's dataset plugins deliver (B,G,R[,A] unless cfg.rgb): converted on the device
   const int channels = img.channels();
   if (img.empty() || img.elemSize1() != 1 || (channels != 1 && channels != 3 && channels != 4)) {
@@ -84,7 +111,8 @@ bool extract(const GSLAM::GImage& img, GSLAM::Svar cfg, std::vector<GSLAM::KeyPo
     std::vector<uint8_t> d((size_t)n * 32);
     int got = n;
     // GImage has no row stride: row i at data + i*cols (GImage.h:378)
-    const int rc = gb_orb_extract_image(ctx, img.data, img.cols, img.rows, channels, rgb, &c, reinterpret_cast<gb_keypoint*>(kps.data()), d.data(), &got);
+    const int rc = remap ? gb_orb_extract_undistorted(ctx, remap, img.data, channels, rgb, &c, reinterpret_cast<gb_keypoint*>(kps.data()), d.data(), &got)
+                         : gb_orb_extract_image(ctx, img.data, img.cols, img.rows, channels, rgb, &c, reinterpret_cast<gb_keypoint*>(kps.data()), d.data(), &got);
     if (rc == GB_ERR_CAPACITY && got > n) { n = got; continue; }
     if (rc != GB_OK) {
       LOG(ERROR) << "gslam_b200 orb_extract: " << gb_last_error(ctx);
@@ -287,12 +315,8 @@ REGISTER_SVAR_MODULE(b200) {
     return out;
   });
   // undistort(image, camera_in, camera_out) -> image: GSLAM::Undistorter::undistort (GSLAM/core/Undistorter.h:271-348) with the table
-  // of the reference's own prepareReMap (:120-203; every camera model stays the reference's) applied on the device.  The table of the
-  // last camera pair is kept resident in HBM.
+  // of the reference's own prepareReMap applied on the device (RemapCache).
   svar["gslam"]["b200"]["undistort"] = GSLAM::Svar::lambda([](GSLAM::GImage img, GSLAM::Camera in, GSLAM::Camera out) -> GSLAM::GImage {
-    static std::mutex mtx;
-    static std::string cached_key;
-    static gb_remap* cached_map = nullptr;  // lives as long as the process-wide context it was created on
     if (img.empty() || (img.channels() != 1 && img.channels() != 3) || img.elemSize1() != 1 || !in.isValid() || !out.isValid() ||
         img.cols != in.width() || img.rows != in.height()) {
       LOG(ERROR) << "gslam_b200 undistort: needs an 8-bit 1- or 3-channel image of camera_in's size and two valid cameras";
@@ -300,25 +324,43 @@ REGISTER_SVAR_MODULE(b200) {
     }
     gb_ctx* ctx = shared().get();
     if (!ctx) return GSLAM::GImage();
-    std::lock_guard<std::mutex> lk(mtx);
-    const std::string key = in.info() + "|" + out.info();
-    if (cached_key != key || !cached_map) {
-      if (cached_map) gb_remap_destroy(ctx, cached_map);
-      cached_map = nullptr;
-      GSLAM::UndistorterImpl table(in, out);
-      if (!table.valid || gb_remap_create(ctx, in.width(), in.height(), out.width(), out.height(), table.remapIdx, table.remapCoef, table.remapX,
-                                          &cached_map) != GB_OK) {
-        LOG(ERROR) << "gslam_b200 undistort: " << gb_last_error(ctx);
-        return GSLAM::GImage();
-      }
-      cached_key = key;
+    std::lock_guard<std::mutex> lk(remaps().mtx);
+    gb_remap* map = remaps().get(ctx, in, out);
+    if (!map) {
+      LOG(ERROR) << "gslam_b200 undistort: " << gb_last_error(ctx);
+      return GSLAM::GImage();
     }
     GSLAM::GImage result(out.height(), out.width(), img.type());
-    if (gb_remap_apply(ctx, cached_map, img.data, img.channels(), result.data) != GB_OK) {
+    if (gb_remap_apply(ctx, map, img.data, img.channels(), result.data) != GB_OK) {
       LOG(ERROR) << "gslam_b200 undistort: " << gb_last_error(ctx);
       return GSLAM::GImage();
     }
     return result;
+  });
+  // orb_extract_undistorted(image, camera_in, camera_out, cfg): orb_extract of undistort(image, camera_in, camera_out) -- converted to
+  // gray as orb_extract converts a colour frame -- without the undistorted frame ever existing on the host: one upload, one
+  // synchronisation.  Keypoints are in camera_out pixels.
+  svar["gslam"]["b200"]["orb_extract_undistorted"] = GSLAM::Svar::lambda([](GSLAM::GImage img, GSLAM::Camera in, GSLAM::Camera out, GSLAM::Svar cfg) -> GSLAM::Svar {
+    if (img.empty() || (img.channels() != 1 && img.channels() != 3) || img.elemSize1() != 1 || !in.isValid() || !out.isValid() ||
+        img.cols != in.width() || img.rows != in.height()) {
+      LOG(ERROR) << "gslam_b200 orb_extract_undistorted: needs an 8-bit 1- or 3-channel image of camera_in's size and two valid cameras";
+      return GSLAM::Svar();
+    }
+    gb_ctx* ctx = shared().get();
+    if (!ctx) return GSLAM::Svar();
+    std::lock_guard<std::mutex> lk(remaps().mtx);
+    gb_remap* map = remaps().get(ctx, in, out);
+    if (!map) {
+      LOG(ERROR) << "gslam_b200 orb_extract_undistorted: " << gb_last_error(ctx);
+      return GSLAM::Svar();
+    }
+    std::vector<GSLAM::KeyPoint> kps;
+    GSLAM::GImage desc;
+    if (!extract(img, cfg, kps, desc, map)) return GSLAM::Svar();
+    GSLAM::Svar res = GSLAM::Svar::object();
+    res["keypoints"] = kps;
+    res["descriptors"] = desc;
+    return res;
   });
   svar["gslam"]["b200"]["vocabulary"] = GSLAM::Svar::lambda([](std::shared_ptr<GSLAM::Vocabulary> src) -> std::shared_ptr<GSLAM::Vocabulary> {
     if (!src) return std::shared_ptr<GSLAM::Vocabulary>();

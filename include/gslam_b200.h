@@ -187,6 +187,28 @@ GB_API int gb_remap_create(gb_ctx* ctx, int w_in, int h_in, int w_out, int h_out
                            const float* remap_x, gb_remap** out);
 GB_API int gb_remap_destroy(gb_ctx* ctx, gb_remap* map);
 GB_API int gb_remap_apply(gb_ctx* ctx, gb_remap* map, const uint8_t* src, int channels, uint8_t* dst);
+/* Device-resident forms.  gb_remap_apply keeps frame buffers inside the map, so a map is used by one gb_remap_apply at a time; the
+ * three calls below only READ the map (whatever they stage lives in the ctx), so one map may serve any number of contexts on the
+ * device it was created on, from any thread, at the same time.  A map of another device is GB_ERR_INVALID.  channels: 1 or 3 -- the
+ * reference's 4-channel branch writes 3-channel pixels (Undistorter.h:336) and is not supported.
+ *
+ * gb_remap_apply_to: undistort into device memory, enqueued on the ctx stream.  src: w_in x h_in pixels at src_pitch bytes per row
+ * (>= w_in*channels), a device pointer (read in place when dense; no host synchronisation) or a host pointer (one synchronisation
+ * after the enqueue, so that the buffer may be reused).  d_dst: device, h_out rows of w_out*channels bytes at dst_pitch
+ * (>= w_out*channels; bytes between are not written).  Same bytes as gb_remap_apply. */
+GB_API int gb_remap_apply_to(gb_ctx* ctx, gb_remap* map, const uint8_t* src, int src_is_device, int src_pitch, int channels,
+                             uint8_t* d_dst, int dst_pitch);
+/* undistort -> (gray) -> extract without the frame leaving the device: the remap writes the undistorted gray image straight into level
+ * 0 of the pyramid, then gb_orb_extract_to's chain runs on it.  img: the map's w_in x h_in input, `pitch` bytes per row, device or
+ * host pointer as in gb_remap_apply_to; rgb_order as gb_orb_extract_image.  The frame the extraction sees, and the pixel grid of the
+ * keypoints, is the map's w_out x h_out output.  The result equals gb_remap_apply, cv2.cvtColor's gray, gb_orb_extract in turn, and
+ * everything that chains behind gb_orb_extract_to (gb_match_features, gb_match_stereo_features, gb_bow_transform_features,
+ * gb_features_count / _download) chains behind this call in the same way. */
+GB_API int gb_orb_extract_undistorted_to(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int img_is_device, int pitch, int channels,
+                                         int rgb_order, const gb_orb_cfg* cfg, gb_features* out);
+/* Host-buffer form: img = w_in*h_in*channels dense bytes; one upload, one synchronisation; kps / desc / *n as gb_orb_extract. */
+GB_API int gb_orb_extract_undistorted(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int channels, int rgb_order,
+                                      const gb_orb_cfg* cfg, gb_keypoint* kps, uint8_t* desc, int* n);
 
 /* ---- bag-of-words transform (SURVEY.md section 8f-4) --------------------------------------------------------------------------------
  * GSLAM::Vocabulary::transform(features, BowVector&, FeatureVector&, levelsup)  (GSLAM/core/Vocabulary.h:1558-1622; tree walk
