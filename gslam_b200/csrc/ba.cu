@@ -1894,8 +1894,9 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   tr.stamp("slab");
 
   // ---- one pinned blob, one H2D ------------------------------------------------------------------------------------------
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + measure.blob + 4096));
-  Slab real{g->slab, (uint8_t*)gb_stage_alloc(ctx, measure.blob)};
+  uint8_t* h_blob;
+  GB_CHECK(gb_stage_take(ctx, {{&h_blob, measure.blob}}));
+  Slab real{g->slab, h_blob};
   layout(real);
   ba_fill_measurements(pb, order, cam_perm, real.host(d.o_uv), real.host(d.c_uv), d.has_info ? real.host(d.o_info) : nullptr);
   g->sorted_to_orig.swap(order);
@@ -2242,6 +2243,19 @@ static bool ba_takes_local4(const gb_ba_graph* g) {
          g->d.np > 0;
 }
 
+// Enqueue the D2H copies of g's T_wc poses (finalized into g->pose_wc_out first) into hp and of its points into hx; a null
+// buffer is skipped.
+static int ba_enqueue_download(gb_ctx* ctx, gb_ba_graph* g, double* hp, double* hx) {
+  const BaDev& d = g->d;
+  if (hp) {
+    ba_finalize_kernel<<<gb_div_up(d.nc, 128), 128, 0, ctx->stream>>>(d.nc, d.pose, g->pose_wc_out);
+    GB_LAUNCH_CHECK(ctx);
+    GB_CUDA(ctx, cudaMemcpyAsync(hp, g->pose_wc_out, (size_t)d.nc * 56, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if (hx) GB_CUDA(ctx, cudaMemcpyAsync(hx, d.pts, (size_t)d.np * 24, cudaMemcpyDeviceToHost, ctx->stream));
+  return GB_OK;
+}
+
 // LM loop of a whole solve, then ONE synchronisation for everything the host wants back: the LM scalars and, for the one-shot
 // host-buffer paths, the final T_wc poses / points (pose_out / pts_out may be null).
 static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt, gb_ba_result* res, double* pose_out, double* pts_out) {
@@ -2296,17 +2310,12 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   GB_CUDA(ctx, cudaEventRecord(ev_e, ctx->stream));
   BaDev& dd = g->d;
   const size_t bp = pose_out ? (size_t)dd.nc * 56 : 0, bx = pts_out ? (size_t)dd.np * 24 : 0;
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bp + bx + sizeof(BaScalars) + 1024));
-  BaScalars* hs = unlocked_wait ? g->h_sc : (BaScalars*)gb_stage_alloc(ctx, sizeof(BaScalars));
-  double* hp = bp ? (double*)gb_stage_alloc(ctx, bp + 8) : nullptr;
-  double* hx = bx ? (double*)gb_stage_alloc(ctx, bx + 8) : nullptr;
+  BaScalars* hs;
+  double *hp, *hx;
+  GB_CHECK(gb_stage_take(ctx, {{&hs, unlocked_wait ? 0 : sizeof(BaScalars)}, {&hp, bp}, {&hx, bx}}));
+  if (unlocked_wait) hs = g->h_sc;
   GB_CUDA(ctx, cudaMemcpyAsync(hs, dd.sc, sizeof(BaScalars), cudaMemcpyDeviceToHost, ctx->stream));
-  if (hp) {
-    ba_finalize_kernel<<<gb_div_up(dd.nc, 128), 128, 0, ctx->stream>>>(dd.nc, dd.pose, g->pose_wc_out);
-    GB_LAUNCH_CHECK(ctx);
-    GB_CUDA(ctx, cudaMemcpyAsync(hp, g->pose_wc_out, bp, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  if (hx) GB_CUDA(ctx, cudaMemcpyAsync(hx, dd.pts, bx, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CHECK(ba_enqueue_download(ctx, g, hp, hx));
   if (unlocked_wait) {
     GB_CUDA(ctx, cudaEventRecord(g->ev_done, ctx->stream));
     cudaError_t done;
@@ -2334,20 +2343,13 @@ int gb_ba_graph_solve(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt, gb_
 int gb_ba_graph_download(gb_ctx* ctx, gb_ba_graph* g, double* cam_pose_wc, double* points) {
   if (!ctx || !g) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  BaDev& d = g->d;
-  const size_t bp = (size_t)d.nc * 56, bx = (size_t)d.np * 24;
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bp + bx + 1024));
-  double* hp = (double*)gb_stage_alloc(ctx, bp + 8);
-  double* hx = (double*)gb_stage_alloc(ctx, bx + 8);
-  if (cam_pose_wc && d.nc > 0) {
-    ba_finalize_kernel<<<gb_div_up(d.nc, 128), 128, 0, ctx->stream>>>(d.nc, d.pose, g->pose_wc_out);
-    GB_LAUNCH_CHECK(ctx);
-    GB_CUDA(ctx, cudaMemcpyAsync(hp, g->pose_wc_out, bp, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  if (points && d.np > 0) GB_CUDA(ctx, cudaMemcpyAsync(hx, d.pts, bx, cudaMemcpyDeviceToHost, ctx->stream));
+  const size_t bp = cam_pose_wc ? (size_t)g->d.nc * 56 : 0, bx = points ? (size_t)g->d.np * 24 : 0;
+  double *hp, *hx;
+  GB_CHECK(gb_stage_take(ctx, {{&hp, bp}, {&hx, bx}}));
+  GB_CHECK(ba_enqueue_download(ctx, g, hp, hx));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (cam_pose_wc && d.nc > 0) memcpy(cam_pose_wc, hp, bp);
-  if (points && d.np > 0) memcpy(points, hx, bx);
+  if (hp) memcpy(cam_pose_wc, hp, bp);
+  if (hx) memcpy(points, hx, bx);
   return GB_OK;
 }
 
@@ -2393,13 +2395,8 @@ static int ba_graph_refresh(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_problem* pb
   const int nc = d.nc, np = d.np, no = d.no;
   for (int k = 0; k < no; ++k) GB_CHECK(ba_check_z(ctx, pb, k));
   const size_t b_pose = (size_t)nc * 56, b_pts = (size_t)np * 24, b_uv = (size_t)no * 16, b_info = d.has_info ? (size_t)no * 24 : 0;
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + b_pose + b_pts + 2 * b_uv + b_info + 4096));
-  double* h_pose = (double*)gb_stage_alloc(ctx, b_pose + 8);
-  double* h_pts = (double*)gb_stage_alloc(ctx, b_pts + 8);
-  double* h_uv = (double*)gb_stage_alloc(ctx, b_uv + 8);
-  double* h_cuv = (double*)gb_stage_alloc(ctx, b_uv + 8);
-  double* h_info = b_info ? (double*)gb_stage_alloc(ctx, b_info) : nullptr;
-  if (!h_pose || !h_pts || !h_uv || !h_cuv || (b_info && !h_info)) { gb_set_error(ctx, "gb_ba: staging exhausted"); return GB_ERR_CUDA; }
+  double *h_pose, *h_pts, *h_uv, *h_cuv, *h_info;
+  GB_CHECK(gb_stage_take(ctx, {{&h_pose, b_pose}, {&h_pts, b_pts}, {&h_uv, b_uv}, {&h_cuv, b_uv}, {&h_info, b_info}}));
   memcpy(h_pose, pb->cam_pose_wc, b_pose);
   memcpy(h_pts, pb->points, b_pts);
   ba_fill_measurements(pb, g->sorted_to_orig, g->cam_perm_h, h_uv, h_cuv, h_info);

@@ -458,7 +458,7 @@ static int ba_sweep_plan(gb_ctx* ctx, gb_ba_graph* g) {
   };
   Slab measure;
   layout(measure);
-  // (pageable staging: this runs in the middle of an API call, where the ctx's pinned staging must not be reserved)
+  // (pageable staging: this runs in the middle of an API call whose pinned staging buffers are still live; see gb_stage_take)
   std::vector<uint8_t> h(measure.blob);
   GB_CUDA(ctx, cudaMalloc(&g->sw_alloc, measure.off));
   Slab real{(uint8_t*)g->sw_alloc, h.data()};

@@ -317,9 +317,9 @@ static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, g
       n, d_count, npad, v->weighting, v->scoring, f_word, f_node, f_weight, in_smem ? nullptr : v->d_keys, (int*)v->d_out,
       (unsigned long long*)(v->d_out + o_words), (float*)(v->d_out + o_val), (unsigned long long*)(v->d_out + o_node), (uint32_t*)(v->d_out + o_feat));
   GB_LAUNCH_CHECK(ctx);
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bytes + 2048));
-  uint8_t* h = (uint8_t*)gb_stage_alloc(ctx, bytes);
-  int* hc = pending ? (int*)gb_stage_alloc(ctx, 2 * sizeof(int)) : nullptr;
+  uint8_t* h;
+  int* hc;
+  GB_CHECK(gb_stage_take(ctx, {{&h, bytes}, {&hc, pending ? 2 * sizeof(int) : 0}}));
   GB_CUDA(ctx, cudaMemcpyAsync(h, v->d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   if (hc) GB_CUDA(ctx, cudaMemcpyAsync(hc, d_count, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -341,8 +341,8 @@ static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, g
 static int bow_upload_run(gb_ctx* ctx, gb_vocabulary* v, const uint8_t* desc, int n, int levelsup, uint64_t* words, float* values,
                           int* n_words, uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
   GB_CHECK(gb_dev_realloc(ctx, (void**)&v->d_feat, &v->feat_cap, (size_t)n * 32));
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + (size_t)n * 32 + 1024));
-  uint8_t* h = (uint8_t*)gb_stage_alloc(ctx, (size_t)n * 32);
+  uint8_t* h;
+  GB_CHECK(gb_stage_take(ctx, {{&h, (size_t)n * 32}}));
   memcpy(h, desc, (size_t)n * 32);
   GB_CUDA(ctx, cudaMemcpyAsync(v->d_feat, h, (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream));
   return bow_run(ctx, v, (const uint4*)v->d_feat, n, nullptr, levelsup, words, values, n_words, fv_node, fv_feat, n_fv);

@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -69,8 +70,21 @@ void gb_set_error(gb_ctx* ctx, const char* fmt, ...);
 int gb_features_resolve(gb_ctx* ctx, gb_features* f, const int* hc, int* n);
 // A ctx on `device` that enqueues on `stream`, which another ctx owns and must outlive it (gb_ctx_destroy leaves it alone).
 int gb_ctx_create_on_stream(int device, cudaStream_t stream, gb_ctx** out);
-int gb_stage_reserve(gb_ctx* ctx, size_t bytes);           // make sure the pinned staging holds >= bytes
-void* gb_stage_alloc(gb_ctx* ctx, size_t bytes);           // bump-allocate from pinned staging (256-B aligned), or nullptr
+// One buffer of the ctx's pinned host staging: *p receives its address (nullptr when bytes == 0).
+struct GbStageBuf {
+  void** p;
+  size_t bytes;
+  template <typename T>
+  GbStageBuf(T** p_, size_t bytes_) : p((void**)p_), bytes(bytes_) {}
+};
+// Takes `bufs` from the ctx's pinned staging, each 256-byte aligned, after what the outermost API call on the ctx has taken so far.
+// When they do not fit, the staging is grown first: the stream is synchronised and the old buffer freed, so every pointer an earlier
+// take of the same outermost call returned is dead.  Buffers that must be live at the same time are therefore taken in ONE call; a
+// nested call may take again only once its caller is done with its own earlier buffers.  GB_ERR_CUDA when the staging cannot grow.
+int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbStageBuf> bufs);
+// Enqueues the copy of `rows` rows of `row_bytes` from src (pitch spitch) to device memory d_dst (pitch dpitch) on the ctx stream:
+// device to device, pinned host memory directly, pageable host memory row by row through the pinned staging (one take).
+int gb_upload_2d(gb_ctx* ctx, void* d_dst, size_t dpitch, const void* src, int src_is_device, size_t spitch, size_t row_bytes, int rows);
 int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes);  // grow-only device buffer
 
 // ---- undistortion in front of the ORB extraction: what remap.cu and orb.cu need of each other --------------------------------------
@@ -168,7 +182,7 @@ struct CtxLock {
 // Releases a ctx that the calling thread holds exactly once (one CtxLock) for the scope of a host wait on the device, so that other
 // threads can enqueue on it meanwhile (gb_ctx_wait_for from a tracking thread while the mapping thread waits for its solve).
 // Nothing of the ctx's pinned staging may be waited on or read across it: another thread's CtxLock restarts the bump allocation and
-// gb_stage_reserve may free and reallocate the staging, so a gb_stage_alloc pointer taken before the unlock is invalid after it.
+// gb_stage_take may free and reallocate the staging, so a staging pointer taken before the unlock is invalid after it.
 struct CtxUnlock {
   gb_ctx* c;
   explicit CtxUnlock(gb_ctx* ctx) : c(ctx) {

@@ -15,10 +15,11 @@ void gb_set_error(gb_ctx* ctx, const char* fmt, ...) {
   g_tls_err = buf;
 }
 
-int gb_stage_reserve(gb_ctx* ctx, size_t bytes) {
+static size_t stage_align(size_t off) { return (off + 255) & ~(size_t)255; }
+
+static int gb_stage_reserve(gb_ctx* ctx, size_t bytes) {
   if (bytes <= ctx->h_stage_bytes) return GB_OK;
-  // only legal while nothing is in flight from the old buffer: callers reserve at the top of an API call
-  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // (nothing may be in flight from the old buffer)
   if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
   ctx->h_stage = nullptr;
   ctx->h_stage_bytes = 0;
@@ -29,11 +30,38 @@ int gb_stage_reserve(gb_ctx* ctx, size_t bytes) {
   return GB_OK;
 }
 
-void* gb_stage_alloc(gb_ctx* ctx, size_t bytes) {
-  size_t off = (ctx->h_stage_off + 255) & ~(size_t)255;
+static void* gb_stage_alloc(gb_ctx* ctx, size_t bytes) {
+  size_t off = stage_align(ctx->h_stage_off);
   if (off + bytes > ctx->h_stage_bytes) return nullptr;
   ctx->h_stage_off = off + bytes;
   return ctx->h_stage + off;
+}
+
+int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbStageBuf> bufs) {
+  size_t end = ctx->h_stage_off;
+  for (const GbStageBuf& b : bufs)
+    if (b.bytes) end = stage_align(end) + b.bytes;
+  GB_CHECK(gb_stage_reserve(ctx, end));  // (a grown staging starts empty: the layout below then fits with room to spare)
+  for (const GbStageBuf& b : bufs) *b.p = b.bytes ? gb_stage_alloc(ctx, b.bytes) : nullptr;
+  return GB_OK;
+}
+
+int gb_upload_2d(gb_ctx* ctx, void* d_dst, size_t dpitch, const void* src, int src_is_device, size_t spitch, size_t row_bytes, int rows) {
+  if (!src_is_device) {
+    cudaPointerAttributes at;
+    const bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
+    cudaGetLastError();
+    if (!pinned) {
+      uint8_t* hs;
+      GB_CHECK(gb_stage_take(ctx, {{&hs, row_bytes * rows}}));
+      for (int y = 0; y < rows; ++y) memcpy(hs + (size_t)y * row_bytes, (const uint8_t*)src + (size_t)y * spitch, row_bytes);
+      src = hs;
+      spitch = row_bytes;
+    }
+  }
+  GB_CUDA(ctx, cudaMemcpy2DAsync(d_dst, dpitch, src, spitch, row_bytes, rows, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                                 ctx->stream));
+  return GB_OK;
 }
 
 int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes) {
@@ -321,8 +349,8 @@ int gb_features_count(gb_ctx* ctx, gb_features* f, int* n) {
 GB_API int gb_dbg_features_set_pending(gb_ctx* ctx, gb_features* f, int count, int status, int expect) {
   if (!ctx || !f || count < 0 || count > f->capacity) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + 1024));
-  int* hc = (int*)gb_stage_alloc(ctx, 2 * sizeof(int));
+  int* hc;
+  GB_CHECK(gb_stage_take(ctx, {{&hc, 2 * sizeof(int)}}));
   hc[0] = count;
   hc[1] = status;
   GB_CUDA(ctx, cudaMemcpyAsync(f->d_count, hc, 2 * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
@@ -339,19 +367,18 @@ int gb_features_upload(gb_ctx* ctx, gb_features* f, const gb_keypoint* kps, cons
     gb_set_error(ctx, "gb_features_upload: %d rows > capacity %d", n, f->capacity);
     return GB_ERR_CAPACITY;
   }
-  size_t need = (size_t)n * 32 + (kps ? (size_t)n * sizeof(gb_keypoint) : 0) + 1024;
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + need));
+  uint8_t* hd;
+  gb_keypoint* hk;
+  int* hc;
+  GB_CHECK(gb_stage_take(ctx, {{&hd, (size_t)n * 32}, {&hk, kps ? (size_t)n * sizeof(gb_keypoint) : 0}, {&hc, 2 * sizeof(int)}}));
   if (n > 0) {
-    uint8_t* hd = (uint8_t*)gb_stage_alloc(ctx, (size_t)n * 32);
     memcpy(hd, desc, (size_t)n * 32);
     GB_CUDA(ctx, cudaMemcpyAsync(f->d_desc, hd, (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream));
     if (kps) {
-      gb_keypoint* hk = (gb_keypoint*)gb_stage_alloc(ctx, (size_t)n * sizeof(gb_keypoint));
       memcpy(hk, kps, (size_t)n * sizeof(gb_keypoint));
       GB_CUDA(ctx, cudaMemcpyAsync(f->d_kps, hk, (size_t)n * sizeof(gb_keypoint), cudaMemcpyHostToDevice, ctx->stream));
     }
   }
-  int* hc = (int*)gb_stage_alloc(ctx, 2 * sizeof(int));
   hc[0] = n;
   hc[1] = 0;
   GB_CUDA(ctx, cudaMemcpyAsync(f->d_count, hc, 2 * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
@@ -383,10 +410,10 @@ int gb_features_download(gb_ctx* ctx, gb_features* f, gb_keypoint* kps, uint8_t*
     }
     if (cnt == 0) return GB_OK;
   }
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + (size_t)rows * 60 + 1024));
-  int* hc = (int*)gb_stage_alloc(ctx, 16);
-  gb_keypoint* hk = kps ? (gb_keypoint*)gb_stage_alloc(ctx, (size_t)rows * sizeof(gb_keypoint)) : nullptr;
-  uint8_t* hd = desc ? (uint8_t*)gb_stage_alloc(ctx, (size_t)rows * 32) : nullptr;
+  int* hc;
+  gb_keypoint* hk;
+  uint8_t* hd;
+  GB_CHECK(gb_stage_take(ctx, {{&hc, 16}, {&hk, kps ? (size_t)rows * sizeof(gb_keypoint) : 0}, {&hd, desc ? (size_t)rows * 32 : 0}}));
   if (speculative) GB_CUDA(ctx, cudaMemcpyAsync(hc, f->d_count, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   if (hk && rows > 0) GB_CUDA(ctx, cudaMemcpyAsync(hk, f->d_kps, (size_t)rows * sizeof(gb_keypoint), cudaMemcpyDeviceToHost, ctx->stream));
   if (hd && rows > 0) GB_CUDA(ctx, cudaMemcpyAsync(hd, f->d_desc, (size_t)rows * 32, cudaMemcpyDeviceToHost, ctx->stream));

@@ -303,20 +303,22 @@ int gb_match_stereo_features(gb_ctx* ctx, gb_features* left, gb_features* right,
                          async ? left->d_train_status : nullptr);
 }
 
+// a temporary feature set of the host-buffer entry points (ctx->tmp_q / tmp_t) that holds at least n rows
+static int match_tmp_ensure(gb_ctx* ctx, gb_features** f, int n) {
+  if (*f && (*f)->capacity >= n) return GB_OK;
+  if (*f) gb_features_destroy(ctx, *f);
+  *f = nullptr;
+  return gb_features_create(ctx, n + n / 4 + 64, f);
+}
+
 // Host-buffer variant (what the Svar module's match_stereo binds).
 int gb_match_stereo(gb_ctx* ctx, const gb_keypoint* kps_left, const uint8_t* desc_left, int nl, const gb_keypoint* kps_right, const uint8_t* desc_right,
                     int nr, float band_rows, float min_disparity, float max_disparity, int32_t* best_idx, int32_t* best_dist, int32_t* second_dist) {
   if (!ctx || nl < 0 || nr < 0 || (nl > 0 && (!kps_left || !desc_left)) || (nr > 0 && (!kps_right || !desc_right))) return GB_ERR_INVALID;
   if (nl == 0) return GB_OK;
   CtxLock lk(ctx);
-  auto ensure = [&](gb_features** f, int n) -> int {
-    if (*f && (*f)->capacity >= n) return GB_OK;
-    if (*f) gb_features_destroy(ctx, *f);
-    *f = nullptr;
-    return gb_features_create(ctx, n + n / 4 + 64, f);
-  };
-  GB_CHECK(ensure(&ctx->tmp_q, nl));
-  GB_CHECK(ensure(&ctx->tmp_t, nr > 0 ? nr : 1));
+  GB_CHECK(match_tmp_ensure(ctx, &ctx->tmp_q, nl));
+  GB_CHECK(match_tmp_ensure(ctx, &ctx->tmp_t, nr > 0 ? nr : 1));
   GB_CHECK(gb_features_upload(ctx, ctx->tmp_q, kps_left, desc_left, nl));
   GB_CHECK(gb_features_upload(ctx, ctx->tmp_t, nr > 0 ? kps_right : nullptr, nr > 0 ? desc_right : desc_left, nr));
   GB_CHECK(gb_match_stereo_features(ctx, ctx->tmp_q, ctx->tmp_t, band_rows, min_disparity, max_disparity));
@@ -332,8 +334,8 @@ int gb_match_download(gb_ctx* ctx, gb_features* fq, int32_t* best_idx, int32_t* 
     // copied next to them, come back in one synchronisation.  After a failed extraction every call fails the same way, instead of
     // the second reporting the count the failure left behind (0 matches, or more rows than the feature set holds), and instead of
     // a failed train set reading as an empty one (-1 / 257 / 257 for every query).
-    GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + 1024));
-    int* hs = (int*)gb_stage_alloc(ctx, 4 * sizeof(int));
+    int* hs;
+    GB_CHECK(gb_stage_take(ctx, {{&hs, 4 * sizeof(int)}}));
     GB_CUDA(ctx, cudaMemcpyAsync(hs, fq->d_count, 3 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     int nq = fq->h_count;
@@ -357,10 +359,8 @@ int gb_match_download(gb_ctx* ctx, gb_features* fq, int32_t* best_idx, int32_t* 
   }
   if (cnt == 0) return GB_OK;
   const size_t bytes = (size_t)cnt * sizeof(int32_t);
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + 3 * bytes + 1024));
-  int32_t* h0 = (int32_t*)gb_stage_alloc(ctx, bytes);
-  int32_t* h1 = (int32_t*)gb_stage_alloc(ctx, bytes);
-  int32_t* h2 = (int32_t*)gb_stage_alloc(ctx, bytes);
+  int32_t *h0, *h1, *h2;
+  GB_CHECK(gb_stage_take(ctx, {{&h0, bytes}, {&h1, bytes}, {&h2, bytes}}));
   if (best_idx) GB_CUDA(ctx, cudaMemcpyAsync(h0, fq->d_best, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   if (best_dist) GB_CUDA(ctx, cudaMemcpyAsync(h1, fq->d_dist, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   if (second_dist) GB_CUDA(ctx, cudaMemcpyAsync(h2, fq->d_dist2, bytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -376,22 +376,15 @@ int gb_match_hamming(gb_ctx* ctx, const uint8_t* query, int nq, const uint8_t* t
   if (!ctx || nq < 0 || nt < 0 || (nq > 0 && !query) || (nt > 0 && !train)) return GB_ERR_INVALID;
   if (nq == 0) return GB_OK;
   CtxLock lk(ctx);
-  auto ensure = [&](gb_features** f, int n) -> int {
-    if (*f && (*f)->capacity >= n) return GB_OK;
-    if (*f) gb_features_destroy(ctx, *f);
-    *f = nullptr;
-    return gb_features_create(ctx, n + n / 4 + 64, f);
-  };
-  GB_CHECK(ensure(&ctx->tmp_q, nq));
-  GB_CHECK(ensure(&ctx->tmp_t, nt > 0 ? nt : 1));
+  GB_CHECK(match_tmp_ensure(ctx, &ctx->tmp_q, nq));
+  GB_CHECK(match_tmp_ensure(ctx, &ctx->tmp_t, nt > 0 ? nt : 1));
   gb_features *fq = ctx->tmp_q, *ft = ctx->tmp_t;
-  const size_t bq = (size_t)nq * 32, bt = (size_t)nt * 32, bo = (size_t)nq * sizeof(int32_t);
-  GB_CHECK(gb_stage_reserve(ctx, bq + bt + 3 * bo + 4096));
-  uint8_t* hq = (uint8_t*)gb_stage_alloc(ctx, bq);
+  const size_t bq = (size_t)nq * 32, bt = (size_t)nt * 32;
+  uint8_t *hq, *ht;
+  GB_CHECK(gb_stage_take(ctx, {{&hq, bq}, {&ht, bt}}));
   memcpy(hq, query, bq);
   GB_CUDA(ctx, cudaMemcpyAsync(fq->d_desc, hq, bq, cudaMemcpyHostToDevice, ctx->stream));
   if (nt > 0) {
-    uint8_t* ht = (uint8_t*)gb_stage_alloc(ctx, bt);
     memcpy(ht, train, bt);
     GB_CUDA(ctx, cudaMemcpyAsync(ft->d_desc, ht, bt, cudaMemcpyHostToDevice, ctx->stream));
   }
@@ -399,17 +392,8 @@ int gb_match_hamming(gb_ctx* ctx, const uint8_t* query, int nq, const uint8_t* t
   ft->h_count = nt;
   fq->n_matched = nq;
   GB_CHECK(gb_match_launch(ctx, fq->d_desc, nq, ft->d_desc, nt, fq->d_best, fq->d_dist, fq->d_dist2));
-  int32_t* h0 = (int32_t*)gb_stage_alloc(ctx, bo);
-  int32_t* h1 = (int32_t*)gb_stage_alloc(ctx, bo);
-  int32_t* h2 = (int32_t*)gb_stage_alloc(ctx, bo);
-  if (best_idx) GB_CUDA(ctx, cudaMemcpyAsync(h0, fq->d_best, bo, cudaMemcpyDeviceToHost, ctx->stream));
-  if (best_dist) GB_CUDA(ctx, cudaMemcpyAsync(h1, fq->d_dist, bo, cudaMemcpyDeviceToHost, ctx->stream));
-  if (second_dist) GB_CUDA(ctx, cudaMemcpyAsync(h2, fq->d_dist2, bo, cudaMemcpyDeviceToHost, ctx->stream));
-  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (best_idx) memcpy(best_idx, h0, bo);
-  if (best_dist) memcpy(best_dist, h1, bo);
-  if (second_dist) memcpy(second_dist, h2, bo);
-  return GB_OK;
+  int n = nq;
+  return gb_match_download(ctx, fq, best_idx, best_dist, second_dist, &n);
 }
 
 }  // extern "C"

@@ -879,30 +879,11 @@ static int orb_launch(gb_ctx* ctx, gb_features* out) {
   return GB_OK;
 }
 
-// Copy a frame into the dense frame buffer of the ctx's ORB state (d_color): pinned caller memory goes straight over PCIe, pageable
-// memory is staged through the ctx's pinned buffer.
+// Copy a frame into the dense frame buffer of the ctx's ORB state (d_color).
 static int orb_stage_copy(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row, int height, int pitch) {
   OrbState* s = ctx->orb;
-  const size_t bytes = row * height;
-  GB_CHECK(gb_dev_realloc(ctx, &s->d_color, &s->color_cap, bytes));
-  if (img_is_device) {
-    GB_CUDA(ctx, cudaMemcpy2DAsync(s->d_color, row, img, pitch, row, height, cudaMemcpyDeviceToDevice, ctx->stream));
-    return GB_OK;
-  }
-  cudaPointerAttributes at;
-  const bool pinned = cudaPointerGetAttributes(&at, img) == cudaSuccess && at.type == cudaMemoryTypeHost;
-  cudaGetLastError();
-  const uint8_t* src = img;
-  size_t spitch = (size_t)pitch;
-  if (!pinned) {
-    GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + bytes + 1024));
-    uint8_t* hs = (uint8_t*)gb_stage_alloc(ctx, bytes);
-    for (int y = 0; y < height; ++y) memcpy(hs + (size_t)y * row, img + (size_t)y * pitch, row);
-    src = hs;
-    spitch = row;
-  }
-  GB_CUDA(ctx, cudaMemcpy2DAsync(s->d_color, row, src, spitch, row, height, cudaMemcpyHostToDevice, ctx->stream));
-  return GB_OK;
+  GB_CHECK(gb_dev_realloc(ctx, &s->d_color, &s->color_cap, row * height));
+  return gb_upload_2d(ctx, s->d_color, row, img, img_is_device, pitch, row, height);
 }
 
 int gb_orb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row_bytes, int height, int pitch, const uint8_t** d_frame) {
@@ -950,23 +931,8 @@ static int orb_extract_to_impl(gb_ctx* ctx, const uint8_t* img, int img_is_devic
     orb_gray_kernel<<<dim3(gb_div_up(width, 256), height), 256, 0, ctx->stream>>>((const uint8_t*)s->d_color, width, height, channels, rgb_order,
                                                                                  s->d_pyr + L0.off, L0.pitch);
     GB_LAUNCH_CHECK(ctx);
-  } else if (img_is_device) {
-    GB_CUDA(ctx, cudaMemcpy2DAsync(s->d_pyr + L0.off, L0.pitch, img, pitch, width, height, cudaMemcpyDeviceToDevice, ctx->stream));
   } else {
-    // pinned caller memory goes straight over PCIe; pageable memory is staged through the ctx's pinned buffer
-    cudaPointerAttributes at;
-    const bool pinned = cudaPointerGetAttributes(&at, img) == cudaSuccess && at.type == cudaMemoryTypeHost;
-    cudaGetLastError();
-    const uint8_t* src = img;
-    int spitch = pitch;
-    if (!pinned) {
-      GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + (size_t)width * height + 1024));
-      uint8_t* hs = (uint8_t*)gb_stage_alloc(ctx, (size_t)width * height);
-      for (int y = 0; y < height; ++y) memcpy(hs + (size_t)y * width, img + (size_t)y * pitch, width);
-      src = hs;
-      spitch = width;
-    }
-    GB_CUDA(ctx, cudaMemcpy2DAsync(s->d_pyr + L0.off, L0.pitch, src, spitch, width, height, cudaMemcpyHostToDevice, ctx->stream));
+    GB_CHECK(gb_upload_2d(ctx, s->d_pyr + L0.off, L0.pitch, img, img_is_device, pitch, width, height));
   }
   GB_CHECK(orb_launch(ctx, out));
   if (!img_is_device && sync_after) GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staging / caller buffer may be reused

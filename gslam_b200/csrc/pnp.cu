@@ -318,12 +318,9 @@ int pnp_run_hypotheses(gb_ctx* ctx, int n, const double* xyz, const double* xy, 
   int* d_cnt = (int*)base; base += al(b_cnt);
   int* d_root = (int*)base; base += al(b_cnt);
   double* d_Rt = (double*)base;
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + b_xyz + b_xy + 2 * b_cnt + 4096));
-  double* h_xyz = (double*)gb_stage_alloc(ctx, b_xyz);
-  double* h_xy = (double*)gb_stage_alloc(ctx, b_xy);
-  int* h_cnt = (int*)gb_stage_alloc(ctx, b_cnt);
-  int* h_root = (int*)gb_stage_alloc(ctx, b_cnt);
-  if (!h_xyz || !h_xy || !h_cnt || !h_root) { gb_set_error(ctx, "gb_pnp_ransac: staging exhausted"); return GB_ERR_CUDA; }
+  double *h_xyz, *h_xy;
+  int *h_cnt, *h_root;
+  GB_CHECK(gb_stage_take(ctx, {{&h_xyz, b_xyz}, {&h_xy, b_xy}, {&h_cnt, b_cnt}, {&h_root, b_cnt}}));
   memcpy(h_xyz, xyz, b_xyz);
   memcpy(h_xy, xy, b_xy);
   GB_CUDA(ctx, cudaMemcpyAsync(d_xyz, h_xyz, b_xyz, cudaMemcpyHostToDevice, ctx->stream));

@@ -161,9 +161,8 @@ int gb_remap_apply(gb_ctx* ctx, gb_remap* m, const uint8_t* src, int channels, u
   const size_t n_in = (size_t)m->w_in * m->h_in, n_out = (size_t)m->w_out * m->h_out, b_in = n_in * channels, b_out = n_out * channels;
   GB_CHECK(gb_dev_realloc(ctx, (void**)&m->d_src, &m->src_cap, b_in));
   GB_CHECK(gb_dev_realloc(ctx, (void**)&m->d_dst, &m->dst_cap, b_out));
-  GB_CHECK(gb_stage_reserve(ctx, ctx->h_stage_off + b_in + b_out + 1024));
-  uint8_t* hs = (uint8_t*)gb_stage_alloc(ctx, b_in);
-  uint8_t* hd = (uint8_t*)gb_stage_alloc(ctx, b_out);
+  uint8_t *hs, *hd;
+  GB_CHECK(gb_stage_take(ctx, {{&hs, b_in}, {&hd, b_out}}));
   memcpy(hs, src, b_in);
   GB_CUDA(ctx, cudaMemcpyAsync(m->d_src, hs, b_in, cudaMemcpyHostToDevice, ctx->stream));
   remap_kernel<<<gb_div_up((int)n_out, 256), 256, 0, ctx->stream>>>((const int4*)m->d_idx, (const float4*)m->d_coef, m->d_x, (int)n_out, (int)n_in, channels,
