@@ -249,11 +249,13 @@ class Remap:
         ctx._check(ctx._lib.gb_remap_create(ctx._h, w_in, h_in, w_out, h_out, ptr(idx4), ptr(coef4), ptr(rx), C.byref(h)))
         self._h = h
 
-    def apply(self, img: np.ndarray) -> np.ndarray:
+    def apply(self, img: np.ndarray, ctx: Context | None = None) -> np.ndarray:
+        """Undistort a host frame on the stream of `ctx` (default: the map's own)."""
+        c = ctx or self.ctx
         img = np.ascontiguousarray(img, np.uint8)
         ch = 1 if img.ndim == 2 else img.shape[2]
         out = np.zeros(self.shape_out + ((ch,) if img.ndim == 3 else ()), np.uint8)
-        self.ctx._check(self.ctx._lib.gb_remap_apply(self.ctx._h, self._h, ptr(img), ch, ptr(out)))
+        c._check(c._lib.gb_remap_apply(c._h, self._h, ptr(img), ch, ptr(out)))
         return out
 
     def _channels(self, img: np.ndarray) -> int:

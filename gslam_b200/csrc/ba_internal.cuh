@@ -2,35 +2,10 @@
 // (ba.cu: graph upload, kernels of the sweep / Schur / local PCG paths; ba_pcg_bcsr.cu: the multi-CTA block-CSR PCG of large
 // reduced systems; ba_dist.cu: the landmark-sharded multi-GPU solve and its communicator).  Not part of the C-ABI.
 #pragma once
-#include <type_traits>
 #include <vector>
 
 #include "ba_device.cuh"
 #include "common.cuh"
-
-// Layout of one device allocation, written as ONE list of declarations that is run twice: first to measure (base == nullptr),
-// then to place the arrays at base.  put() declares an uploaded array and copies its host source, if it has one, into the pinned
-// staging h at the array's offset; the puts come first, so [0, blob) is one contiguous upload.  take() declares device-only
-// working memory after them.  Every array starts on a 256-byte boundary (kernels such as cta_copy_f64 rely on it).
-struct Slab {
-  uint8_t* base = nullptr;
-  uint8_t* h = nullptr;  // host staging mirror of [0, blob)
-  size_t off = 0, blob = 0;
-  template <typename T>
-  void take(T** p, size_t n) {
-    off = (off + 255) & ~(size_t)255;
-    if (base) *p = (T*)(base + off);
-    off += std::max<size_t>(n, 1) * sizeof(T);
-  }
-  template <typename T>
-  void put(T** p, size_t n, const std::remove_const_t<T>* src = nullptr) {
-    take(p, n);
-    blob = off;
-    if (h && src && n) memcpy(h + ((const uint8_t*)*p - base), src, n * sizeof(T));
-  }
-  template <typename T>
-  std::remove_const_t<T>* host(T* p) const { return (std::remove_const_t<T>*)(h + ((const uint8_t*)p - base)); }  // staging of a put array
-};
 
 // host-made plans of graph creation, uploaded with the graph (ba_graph_create_impl lays them out)
 struct BaSchurPlan {  // landmark-chunk Schur complement: BaDev::sp_*

@@ -19,22 +19,18 @@
 // ascending word order, as the reference does.  L1 norms of idf-like weights stay far inside the bound; L2 norms of weights that
 // span many octaves (squares keep 24 significant bits over twice the span) can leave it, and then the sequential sum runs.
 // A leaf met above level L - levelsup leaves the reference's node id uninitialised (:1579,1728); it files under the leaf itself here.
-// One vocabulary may be used from any ctx on its device, from any thread: its per-call scratch is guarded by its own lock, held
-// until the call's stream is synchronised.
+// One vocabulary may be used from any ctx on its device, from any thread, at the same time: it is immutable after creation (but for
+// the plan of the last call, a test hook), and every call's working memory is its ctx's device scratch.
 #include "common.cuh"
 
 struct gb_vocabulary {
   int k = 0, L = 0, weighting = 0, scoring = 0;
   uint32_t n_nodes = 0;
+  void* d_slab = nullptr;       // one allocation holding the three arrays below
   uint32_t* d_child = nullptr;  // [n_nodes]
   float* d_weight = nullptr;    // [n_nodes]
   uint4* d_desc = nullptr;      // [n_nodes][2]
-  std::mutex mu;                // guards everything below across a whole transform (the callers' ctxs may differ)
-  // per-call scratch (grow-only): per-feature word / node / weight, sorted keys (large inputs), outputs
-  uint8_t* d_feat = nullptr; size_t feat_cap = 0;
-  uint32_t* d_fword = nullptr; size_t fword_cap = 0;  // [n] word, [n] node, [n] weight bits
-  unsigned long long* d_keys = nullptr; size_t keys_cap = 0;  // [2][npad] when the keys do not fit shared memory
-  uint8_t* d_out = nullptr; size_t out_cap = 0;       // [counts(4 ints) | words u64[n] | fv_node u64[n] | values f32[n] | fv_feat u32[n]]
+  std::mutex mu;                // guards last_plan (the callers' ctxs may differ)
   int last_plan[5] = {0, 0, 0, 0, 0};  // of the last launch (gb_dbg_bow_last_plan): G, keys in smem, npad launched, npad sorted, flags
 };
 
@@ -269,18 +265,20 @@ int gb_voc_create(gb_ctx* ctx, int k, int L, int weighting, int scoring, uint32_
   CtxLock lk(ctx);
   gb_vocabulary* v = new gb_vocabulary();
   v->k = k; v->L = L; v->weighting = weighting; v->scoring = scoring; v->n_nodes = n_nodes;
-  cudaError_t e = cudaMalloc((void**)&v->d_child, (size_t)n_nodes * 4);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&v->d_weight, (size_t)n_nodes * 4);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&v->d_desc, (size_t)n_nodes * 32);
-  if (e == cudaSuccess) e = cudaMemcpy(v->d_child, child_num, (size_t)n_nodes * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(v->d_weight, weight, (size_t)n_nodes * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(v->d_desc, desc32, (size_t)n_nodes * 32, cudaMemcpyHostToDevice);
-  const bool smem_ok = e == cudaSuccess && gb_func_setup(ctx, (const void*)bow_reduce_kernel, 2 * kSmemKeys * (int)sizeof(unsigned long long));
-  if (!smem_ok) {
+  const size_t n = n_nodes;
+  int rc = gb_slab_alloc(ctx, &v->d_slab, [&](Slab& sl) { sl.take(&v->d_child, n); sl.take(&v->d_weight, n); sl.take(&v->d_desc, 2 * n); });
+  cudaError_t e = cudaSuccess;
+  if (rc == GB_OK) e = cudaMemcpy(v->d_child, child_num, n * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(v->d_weight, weight, n * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(v->d_desc, desc32, n * 32, cudaMemcpyHostToDevice);
+  if (rc == GB_OK && (e != cudaSuccess || !gb_func_setup(ctx, (const void*)bow_reduce_kernel, 2 * kSmemKeys * (int)sizeof(unsigned long long)))) {
     gb_set_error(ctx, "gb_voc_create -> %s", e != cudaSuccess ? cudaGetErrorString(e) : "cannot set the shared-memory limit of the reduce kernel");
-    cudaFree(v->d_child); cudaFree(v->d_weight); cudaFree(v->d_desc);
+    rc = GB_ERR_CUDA;
+  }
+  if (rc != GB_OK) {
+    cudaFree(v->d_slab);
     delete v;
-    return GB_ERR_CUDA;
+    return rc;
   }
   *out = v;
   return GB_OK;
@@ -289,41 +287,55 @@ int gb_voc_create(gb_ctx* ctx, int k, int L, int weighting, int scoring, uint32_
 int gb_voc_destroy(gb_ctx* ctx, gb_vocabulary* v) {
   if (!v) return GB_OK;
   if (ctx) { CtxLock lk(ctx); cudaStreamSynchronize(ctx->stream); }
-  cudaFree(v->d_child); cudaFree(v->d_weight); cudaFree(v->d_desc); cudaFree(v->d_feat); cudaFree(v->d_fword); cudaFree(v->d_keys); cudaFree(v->d_out);
+  cudaFree(v->d_slab);
   delete v;
   return GB_OK;
 }
 
-// pending (nullable): the feature set of an extraction in flight whose rows d_feats are -- the walk is clipped by its device-side
-// count, and its status word comes back with the results: a failed extraction fails the call instead of reading as an empty frame.
-static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, gb_features* pending, int levelsup, uint64_t* words, float* values,
-                   int* n_words, uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
-  for (int& x : v->last_plan) x = 0;
+static void bow_set_plan(gb_vocabulary* v, const int (&plan)[5]) {
+  std::lock_guard<std::mutex> vl(v->mu);
+  memcpy(v->last_plan, plan, sizeof plan);
+}
+
+// Descriptors: h_desc (host, uploaded through the ctx's staging) or d_feats (device).  pending (nullable): the feature set of an
+// extraction in flight whose rows d_feats are -- the walk is clipped by its device-side count, and its status word comes back with the
+// results: a failed extraction fails the call instead of reading as an empty frame.
+static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint8_t* h_desc, const uint4* d_feats, int n, gb_features* pending, int levelsup,
+                   uint64_t* words, float* values, int* n_words, uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
+  bow_set_plan(v, {0, 0, 0, 0, 0});
   if (n == 0) { *n_words = 0; *n_fv = 0; return GB_OK; }
   const int* d_count = pending ? pending->d_count : nullptr;
   const int npad = next_pow2(n);
   const bool in_smem = npad <= kSmemKeys;
-  GB_CHECK(gb_dev_realloc(ctx, (void**)&v->d_fword, &v->fword_cap, (size_t)n * 12));
-  if (!in_smem) GB_CHECK(gb_dev_realloc(ctx, (void**)&v->d_keys, &v->keys_cap, (size_t)npad * 16));
   const size_t o_words = 16, o_node = o_words + (size_t)n * 8, o_val = o_node + (size_t)n * 8, o_feat = o_val + (size_t)n * 4, bytes = o_feat + (size_t)n * 4;
-  GB_CHECK(gb_dev_realloc(ctx, (void**)&v->d_out, &v->out_cap, bytes));
-  uint32_t* f_word = v->d_fword; uint32_t* f_node = f_word + n; float* f_weight = (float*)(f_node + n);
+  uint8_t *d_feat, *d_out;
+  uint32_t* f_word;  // [n] word, [n] node, [n] weight bits
+  unsigned long long* d_keys;  // [2][npad] when the keys do not fit shared memory
+  GB_CHECK(gb_scratch_take(ctx, {{&d_feat, h_desc ? (size_t)n * 32 : 0}, {&f_word, (size_t)n * 12}, {&d_keys, in_smem ? 0 : (size_t)npad * 16}, {&d_out, bytes}}));
+  if (h_desc) {
+    uint8_t* h;
+    GB_CHECK(gb_stage_take(ctx, {{&h, (size_t)n * 32}}));
+    memcpy(h, h_desc, (size_t)n * 32);
+    GB_CUDA(ctx, cudaMemcpyAsync(d_feat, h, (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream));
+    d_feats = (const uint4*)d_feat;
+  }
+  uint32_t* f_node = f_word + n; float* f_weight = (float*)(f_node + n);
   const int G = v->k <= 16 ? 16 : 32;
   const int blocks = gb_div_up(n * G, kWalkThreads);
   if (G == 16) bow_walk_kernel<16><<<blocks, kWalkThreads, 0, ctx->stream>>>(v->k, v->L, v->d_child, v->d_weight, v->d_desc, d_feats, n, d_count, levelsup, f_word, f_node, f_weight);
   else bow_walk_kernel<32><<<blocks, kWalkThreads, 0, ctx->stream>>>(v->k, v->L, v->d_child, v->d_weight, v->d_desc, d_feats, n, d_count, levelsup, f_word, f_node, f_weight);
   GB_LAUNCH_CHECK(ctx);
   bow_reduce_kernel<<<1, kRedThreads, in_smem ? (size_t)npad * 16 : 0, ctx->stream>>>(
-      n, d_count, npad, v->weighting, v->scoring, f_word, f_node, f_weight, in_smem ? nullptr : v->d_keys, (int*)v->d_out,
-      (unsigned long long*)(v->d_out + o_words), (float*)(v->d_out + o_val), (unsigned long long*)(v->d_out + o_node), (uint32_t*)(v->d_out + o_feat));
+      n, d_count, npad, v->weighting, v->scoring, f_word, f_node, f_weight, in_smem ? nullptr : d_keys, (int*)d_out,
+      (unsigned long long*)(d_out + o_words), (float*)(d_out + o_val), (unsigned long long*)(d_out + o_node), (uint32_t*)(d_out + o_feat));
   GB_LAUNCH_CHECK(ctx);
   uint8_t* h;
   int* hc;
   GB_CHECK(gb_stage_take(ctx, {{&h, bytes}, {&hc, pending ? 2 * sizeof(int) : 0}}));
-  GB_CUDA(ctx, cudaMemcpyAsync(h, v->d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(h, d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   if (hc) GB_CUDA(ctx, cudaMemcpyAsync(hc, d_count, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  v->last_plan[0] = G; v->last_plan[1] = in_smem; v->last_plan[2] = npad; v->last_plan[3] = ((int*)h)[2]; v->last_plan[4] = ((int*)h)[3];
+  bow_set_plan(v, {G, in_smem, npad, ((int*)h)[2], ((int*)h)[3]});
   if (hc) {
     int cnt = 0;
     const int rc = gb_features_resolve(ctx, pending, hc, &cnt);
@@ -338,40 +350,20 @@ static int bow_run(gb_ctx* ctx, gb_vocabulary* v, const uint4* d_feats, int n, g
   return GB_OK;
 }
 
-static int bow_upload_run(gb_ctx* ctx, gb_vocabulary* v, const uint8_t* desc, int n, int levelsup, uint64_t* words, float* values,
-                          int* n_words, uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
-  GB_CHECK(gb_dev_realloc(ctx, (void**)&v->d_feat, &v->feat_cap, (size_t)n * 32));
-  uint8_t* h;
-  GB_CHECK(gb_stage_take(ctx, {{&h, (size_t)n * 32}}));
-  memcpy(h, desc, (size_t)n * 32);
-  GB_CUDA(ctx, cudaMemcpyAsync(v->d_feat, h, (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream));
-  return bow_run(ctx, v, (const uint4*)v->d_feat, n, nullptr, levelsup, words, values, n_words, fv_node, fv_feat, n_fv);
-}
-
-// A call that failed half way may leave work on the scratch in flight: it must end before the vocabulary's lock is released.
-static int bow_finish(gb_ctx* ctx, int rc) {
-  if (rc != GB_OK) cudaStreamSynchronize(ctx->stream);
-  return rc;
-}
-
 int gb_bow_transform(gb_ctx* ctx, gb_vocabulary* v, const uint8_t* desc, int n, int levelsup, uint64_t* words, float* values, int* n_words,
                      uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
   if (!ctx || !v || n < 0 || (n > 0 && !desc) || !words || !values || !n_words || !fv_node || !fv_feat || !n_fv) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  std::lock_guard<std::mutex> vl(v->mu);
-  if (n == 0) { for (int& x : v->last_plan) x = 0; *n_words = 0; *n_fv = 0; return GB_OK; }
-  return bow_finish(ctx, bow_upload_run(ctx, v, desc, n, levelsup, words, values, n_words, fv_node, fv_feat, n_fv));
+  return bow_run(ctx, v, desc, nullptr, n, nullptr, levelsup, words, values, n_words, fv_node, fv_feat, n_fv);
 }
 
 int gb_bow_transform_features(gb_ctx* ctx, gb_vocabulary* v, gb_features* f, int levelsup, uint64_t* words, float* values, int* n_words,
                               uint64_t* fv_node, uint32_t* fv_feat, int* n_fv) {
   if (!ctx || !v || !f || !words || !values || !n_words || !fv_node || !fv_feat || !n_fv) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  std::lock_guard<std::mutex> vl(v->mu);
   // the descriptors of an extraction still in flight: the launch is sized for the capacity and clipped by the device-side count
   const int n = f->h_count >= 0 ? f->h_count : f->capacity;
-  return bow_finish(ctx, bow_run(ctx, v, (const uint4*)f->d_desc, n, f->h_count >= 0 ? nullptr : f, levelsup, words, values, n_words, fv_node,
-                                 fv_feat, n_fv));
+  return bow_run(ctx, v, nullptr, (const uint4*)f->d_desc, n, f->h_count >= 0 ? nullptr : f, levelsup, words, values, n_words, fv_node, fv_feat, n_fv);
 }
 
 // test hook: the plan of the last transform with this vocabulary -- {lanes per descriptor, keys in shared memory, keys launched,

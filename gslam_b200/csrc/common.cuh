@@ -6,15 +6,23 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <algorithm>
 #include <initializer_list>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/gslam_b200.h"
 
 struct OrbState;    // orb.cu
 struct MatchState;  // match.cu
+
+// A grow-only buffer that one outermost API call on a ctx bump-allocates and CtxLock resets: the pinned staging, the device scratch.
+struct GbBump {
+  uint8_t* base = nullptr;
+  size_t bytes = 0, off = 0;
+};
 
 struct gb_ctx {
   int device = 0;
@@ -28,11 +36,10 @@ struct gb_ctx {
   std::recursive_mutex mu;
   std::string err;
   int64_t launches = 0;
-  // pinned host staging (bump-allocated inside one API call, reset at its end)
-  uint8_t* h_stage = nullptr;
-  size_t h_stage_bytes = 0, h_stage_off = 0;
+  GbBump stage;    // pinned host staging (gb_stage_take)
+  GbBump scratch;  // device scratch (gb_scratch_take)
   int lock_depth = 0;
-  // generic device scratch owned by subsystems
+  // device state owned by subsystems
   OrbState* orb = nullptr;
   MatchState* match = nullptr;
   gb_features* tmp_q = nullptr;  // temporaries of the host-buffer match entry point
@@ -44,12 +51,11 @@ struct gb_ctx {
   gb_ba_graph* ba_cached = nullptr;  // the graph of the last gb_ba_solve, kept (with the arena) while the TOPOLOGY of the calls stays
   void* ba_cache_key = nullptr;      // the same: a sliding window re-solved with new estimates skips sorting / structure / plans
   int ba_last_paths = 0;             // gb_dbg_ba_paths bits of the graph the last gb_ba_solve / gb_ba_pnp solved (gb_dbg_ba_last_paths)
-  void* pnp_scratch = nullptr;   // grow-only device scratch of gb_pnp_ransac (points, measurements, per-hypothesis results)
-  size_t pnp_scratch_cap = 0;
 };
 
 struct gb_features {
   int capacity = 0;
+  void* d_slab = nullptr;        // the one device allocation holding every array below
   gb_keypoint* d_kps = nullptr;  // [capacity]
   uint8_t* d_desc = nullptr;     // [capacity*32], 32-byte rows
   int* d_count = nullptr;        // device-side keypoint count (written by extract)
@@ -70,28 +76,36 @@ void gb_set_error(gb_ctx* ctx, const char* fmt, ...);
 int gb_features_resolve(gb_ctx* ctx, gb_features* f, const int* hc, int* n);
 // A ctx on `device` that enqueues on `stream`, which another ctx owns and must outlive it (gb_ctx_destroy leaves it alone).
 int gb_ctx_create_on_stream(int device, cudaStream_t stream, gb_ctx** out);
-// One buffer of the ctx's pinned host staging: *p receives its address (nullptr when bytes == 0).
-struct GbStageBuf {
+// One buffer of a take from the ctx's pinned staging or device scratch: *p receives its address (nullptr when bytes == 0).
+struct GbBuf {
   void** p;
   size_t bytes;
   template <typename T>
-  GbStageBuf(T** p_, size_t bytes_) : p((void**)p_), bytes(bytes_) {}
+  GbBuf(T** p_, size_t bytes_) : p((void**)p_), bytes(bytes_) {}
 };
 // Takes `bufs` from the ctx's pinned staging, each 256-byte aligned, after what the outermost API call on the ctx has taken so far.
 // When they do not fit, the staging is grown first: the stream is synchronised and the old buffer freed, so every pointer an earlier
 // take of the same outermost call returned is dead.  Buffers that must be live at the same time are therefore taken in ONE call; a
 // nested call may take again only once its caller is done with its own earlier buffers.  GB_ERR_CUDA when the staging cannot grow.
-int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbStageBuf> bufs);
+int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs);
+// The same for the ctx's grow-only device scratch: the per-call working memory of the host-buffer entry points, the staged frames and
+// the test hooks, so that the long-lived objects they read (maps, vocabularies) stay immutable after creation.  Two rules:
+//  * Take together.  Buffers that must be live at the same time are taken in one call: growing the scratch synchronises the stream
+//    and frees the old buffer, which kills every earlier take of the outermost call (bow_run takes the uploaded descriptors of
+//    gb_bow_transform with its word, key and output buffers).
+//  * No scratch access before gb_pdl_wait().  The next call on the ctx reuses the same bytes, ordered behind this call's kernels only
+//    by the stream, so a kernel launched with programmatic dependent launch must not read or write scratch before that wait
+//    (remap_level0_kernel reads only the map's table before it; every other kernel given scratch is a plain launch).
+int gb_scratch_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs);
 // Enqueues the copy of `rows` rows of `row_bytes` from src (pitch spitch) to device memory d_dst (pitch dpitch) on the ctx stream:
 // device to device, pinned host memory directly, pageable host memory row by row through the pinned staging (one take).
 int gb_upload_2d(gb_ctx* ctx, void* d_dst, size_t dpitch, const void* src, int src_is_device, size_t spitch, size_t row_bytes, int rows);
+// A dense device copy of a frame (`height` rows of `row_bytes`): the frame itself when it is a device pointer with pitch == row_bytes,
+// else a copy in the ctx's device scratch (one take, then gb_upload_2d).
+int gb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row_bytes, int height, int pitch, const uint8_t** d_frame);
 int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes);  // grow-only device buffer
 
-// ---- undistortion in front of the ORB extraction: what remap.cu and orb.cu need of each other --------------------------------------
-// A dense device copy of a frame (`height` rows of `row_bytes`): the frame itself when it is a device pointer with pitch == row_bytes,
-// else a copy in the grow-only frame buffer of the ctx's ORB state (cudaMemcpy2DAsync on the ctx stream; pinned host memory directly,
-// pageable host memory through the ctx's pinned staging).  The copy is valid until the next call that stages a frame on this ctx.
-int gb_orb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row_bytes, int height, int pitch, const uint8_t** d_frame);
+// ---- undistortion in front of the ORB extraction: what orb.cu needs of remap.cu ------------------------------------------------------
 void gb_remap_geometry(const gb_remap* m, int* device, int* w_in, int* h_in, int* w_out, int* h_out);
 // Enqueue the remap of the dense device frame d_src (w_in x h_in, 1 or 3 channels) as a GRAY w_out x h_out image at d_dst; d_dst and
 // dst_pitch must be multiples of 4 and dst_pitch >= w_out rounded up to 4 (every word of a row is stored whole).  Reads the map only.
@@ -129,6 +143,44 @@ bool gb_func_setup(gb_ctx* ctx, const void* fn, int smem, bool* nonportable_clus
       return GB_ERR_CUDA;                                                                               \
     }                                                                                                   \
   } while (0)
+
+// Layout of one device allocation, written as ONE list of declarations that is run twice: first to measure (base == nullptr),
+// then to place the arrays at base.  put() declares an uploaded array and copies its host source, if it has one, into the pinned
+// staging h at the array's offset; the puts come first, so [0, blob) is one contiguous upload.  take() declares device-only
+// working memory after them.  Every array starts on a 256-byte boundary (kernels such as cta_copy_f64 rely on it).
+struct Slab {
+  uint8_t* base = nullptr;
+  uint8_t* h = nullptr;  // host staging mirror of [0, blob)
+  size_t off = 0, blob = 0;
+  template <typename T>
+  void take(T** p, size_t n) {
+    off = (off + 255) & ~(size_t)255;
+    if (base) *p = (T*)(base + off);
+    off += std::max<size_t>(n, 1) * sizeof(T);
+  }
+  template <typename T>
+  void put(T** p, size_t n, const std::remove_const_t<T>* src = nullptr) {
+    take(p, n);
+    blob = off;
+    if (h && src && n) memcpy(h + ((const uint8_t*)*p - base), src, n * sizeof(T));
+  }
+  template <typename T>
+  std::remove_const_t<T>* host(T* p) const { return (std::remove_const_t<T>*)(h + ((const uint8_t*)p - base)); }  // staging of a put array
+};
+
+// Places `layout` (a callable that declares its arrays on the Slab it is given) in ONE new device allocation: runs it to measure,
+// allocates, runs it again to place the arrays there.  *base receives the allocation (cudaFree releases every array at once); the
+// uploads of its puts are the caller's.
+template <typename F>
+int gb_slab_alloc(gb_ctx* ctx, void** base, F&& layout) {
+  Slab sl;
+  layout(sl);
+  *base = nullptr;
+  GB_CUDA(ctx, cudaMalloc(base, sl.off));
+  sl = Slab{(uint8_t*)*base};
+  layout(sl);
+  return GB_OK;
+}
 
 // ---- programmatic dependent launch (sm_90+): a kernel launched with gb_launch_pdl may be scheduled while its predecessor on
 // the stream is still running; it must call gb_pdl_wait() before touching anything the predecessor wrote.  Calling
@@ -170,7 +222,7 @@ struct CtxLock {
     c->mu.lock();
     if (c->lock_depth++ == 0) {
       cudaSetDevice(c->device);
-      c->h_stage_off = 0;
+      c->stage.off = c->scratch.off = 0;
     }
   }
   ~CtxLock() {
@@ -181,8 +233,8 @@ struct CtxLock {
 
 // Releases a ctx that the calling thread holds exactly once (one CtxLock) for the scope of a host wait on the device, so that other
 // threads can enqueue on it meanwhile (gb_ctx_wait_for from a tracking thread while the mapping thread waits for its solve).
-// Nothing of the ctx's pinned staging may be waited on or read across it: another thread's CtxLock restarts the bump allocation and
-// gb_stage_take may free and reallocate the staging, so a staging pointer taken before the unlock is invalid after it.
+// Nothing of the ctx's pinned staging or device scratch may be waited on or read across it: another thread's CtxLock restarts the bump
+// allocation and a take may free and reallocate the buffer, so a pointer taken before the unlock is invalid after it.
 struct CtxUnlock {
   gb_ctx* c;
   explicit CtxUnlock(gb_ctx* ctx) : c(ctx) {

@@ -1,4 +1,4 @@
-// gslam_b200/csrc/ctx.cu — gb_ctx lifetime, error strings, pinned staging, timers, gb_features containers.
+// gslam_b200/csrc/ctx.cu — gb_ctx lifetime, error strings, pinned staging and device scratch, timers, gb_features containers.
 #include <map>
 
 #include "common.cuh"
@@ -15,36 +15,38 @@ void gb_set_error(gb_ctx* ctx, const char* fmt, ...) {
   g_tls_err = buf;
 }
 
-static size_t stage_align(size_t off) { return (off + 255) & ~(size_t)255; }
+static size_t take_align(size_t off) { return (off + 255) & ~(size_t)255; }
 
-static int gb_stage_reserve(gb_ctx* ctx, size_t bytes) {
-  if (bytes <= ctx->h_stage_bytes) return GB_OK;
+// Replaces b's buffer by one of at least `bytes` (device memory or pinned host memory), with room to spare, and empties it.
+static int bump_grow(gb_ctx* ctx, GbBump& b, bool device, size_t bytes) {
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // (nothing may be in flight from the old buffer)
-  if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-  ctx->h_stage = nullptr;
-  ctx->h_stage_bytes = 0;
-  size_t want = bytes + (bytes >> 2) + 4096;
-  GB_CUDA(ctx, cudaHostAlloc((void**)&ctx->h_stage, want, cudaHostAllocDefault));
-  ctx->h_stage_bytes = want;
-  ctx->h_stage_off = 0;
+  if (device) cudaFree(b.base);
+  else cudaFreeHost(b.base);
+  b = GbBump{};
+  const size_t want = device ? bytes + (bytes >> 3) + 256 : bytes + (bytes >> 2) + 4096;
+  GB_CUDA(ctx, device ? cudaMalloc((void**)&b.base, want) : cudaHostAlloc((void**)&b.base, want, cudaHostAllocDefault));
+  b.bytes = want;
   return GB_OK;
 }
 
-static void* gb_stage_alloc(gb_ctx* ctx, size_t bytes) {
-  size_t off = stage_align(ctx->h_stage_off);
-  if (off + bytes > ctx->h_stage_bytes) return nullptr;
-  ctx->h_stage_off = off + bytes;
-  return ctx->h_stage + off;
-}
-
-int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbStageBuf> bufs) {
-  size_t end = ctx->h_stage_off;
-  for (const GbStageBuf& b : bufs)
-    if (b.bytes) end = stage_align(end) + b.bytes;
-  GB_CHECK(gb_stage_reserve(ctx, end));  // (a grown staging starts empty: the layout below then fits with room to spare)
-  for (const GbStageBuf& b : bufs) *b.p = b.bytes ? gb_stage_alloc(ctx, b.bytes) : nullptr;
+static int bump_take(gb_ctx* ctx, GbBump& b, bool device, std::initializer_list<GbBuf> bufs) {
+  size_t end = b.off;
+  for (const GbBuf& x : bufs)
+    if (x.bytes) end = take_align(end) + x.bytes;
+  if (end > b.bytes) GB_CHECK(bump_grow(ctx, b, device, end));  // (a grown buffer starts empty: the layout below then fits)
+  for (const GbBuf& x : bufs) {
+    *x.p = nullptr;
+    if (!x.bytes) continue;
+    b.off = take_align(b.off);
+    *x.p = b.base + b.off;
+    b.off += x.bytes;
+  }
   return GB_OK;
 }
+
+int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs) { return bump_take(ctx, ctx->stage, false, bufs); }
+
+int gb_scratch_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs) { return bump_take(ctx, ctx->scratch, true, bufs); }
 
 int gb_upload_2d(gb_ctx* ctx, void* d_dst, size_t dpitch, const void* src, int src_is_device, size_t spitch, size_t row_bytes, int rows) {
   if (!src_is_device) {
@@ -61,6 +63,18 @@ int gb_upload_2d(gb_ctx* ctx, void* d_dst, size_t dpitch, const void* src, int s
   }
   GB_CUDA(ctx, cudaMemcpy2DAsync(d_dst, dpitch, src, spitch, row_bytes, rows, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
                                  ctx->stream));
+  return GB_OK;
+}
+
+int gb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row_bytes, int height, int pitch, const uint8_t** d_frame) {
+  if (img_is_device && (size_t)pitch == row_bytes) {
+    *d_frame = img;
+    return GB_OK;
+  }
+  uint8_t* d;
+  GB_CHECK(gb_scratch_take(ctx, {{&d, row_bytes * height}}));
+  GB_CHECK(gb_upload_2d(ctx, d, row_bytes, img, img_is_device, pitch, row_bytes, height));
+  *d_frame = d;
   return GB_OK;
 }
 
@@ -184,7 +198,7 @@ static int ctx_create_impl(int device, int high_priority, cudaStream_t borrowed,
     if (ctx->evs) cudaEventDestroy(ctx->evs);
     if (ctx->eve) cudaEventDestroy(ctx->eve);
     if (ctx->stream && ctx->owns_stream) cudaStreamDestroy(ctx->stream);
-    if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
+    if (ctx->stage.base) cudaFreeHost(ctx->stage.base);
     delete ctx;
   };
   if (e != cudaSuccess) {
@@ -192,7 +206,7 @@ static int ctx_create_impl(int device, int high_priority, cudaStream_t borrowed,
     drop();
     return GB_ERR_CUDA;
   }
-  if (gb_stage_reserve(ctx, 8u << 20) != GB_OK) {
+  if (bump_grow(ctx, ctx->stage, false, 8u << 20) != GB_OK) {
     drop();
     return GB_ERR_CUDA;
   }
@@ -211,9 +225,9 @@ int gb_ctx_destroy(gb_ctx* ctx) {
     ba_cache_drop(ctx);
     gb_orb_state_free(ctx);
     gb_match_state_free(ctx);
-    if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
+    if (ctx->stage.base) cudaFreeHost(ctx->stage.base);
+    cudaFree(ctx->scratch.base);
     cudaFree(ctx->ba_arena);
-    cudaFree(ctx->pnp_scratch);
     cudaEventDestroy(ctx->ev0);
     cudaEventDestroy(ctx->ev1);
     cudaEventDestroy(ctx->evs);
@@ -276,18 +290,22 @@ int gb_features_create(gb_ctx* ctx, int capacity, gb_features** out) {
   CtxLock lk(ctx);
   gb_features* f = new gb_features();
   f->capacity = capacity;
-  size_t cap = (size_t)capacity;
-  cudaError_t e = cudaMalloc((void**)&f->d_kps, cap * sizeof(gb_keypoint));
-  if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_desc, cap * 32);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_count, 4 * sizeof(int));  // count, status, train status, (pad)
-  if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_best, cap * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_dist, cap * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMalloc((void**)&f->d_dist2, cap * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMemsetAsync(f->d_count, 0, 4 * sizeof(int), ctx->stream);
-  if (e != cudaSuccess) {
-    gb_set_error(ctx, "gb_features_create(%d) -> %s", capacity, cudaGetErrorString(e));
+  const size_t cap = (size_t)capacity;
+  int rc = gb_slab_alloc(ctx, &f->d_slab, [&](Slab& sl) {
+    sl.take(&f->d_kps, cap);
+    sl.take(&f->d_desc, cap * 32);
+    sl.take(&f->d_count, 4);  // count, status, train status, (pad)
+    sl.take(&f->d_best, cap);
+    sl.take(&f->d_dist, cap);
+    sl.take(&f->d_dist2, cap);
+  });
+  if (rc == GB_OK && cudaMemsetAsync(f->d_count, 0, 4 * sizeof(int), ctx->stream) != cudaSuccess) {
+    gb_set_error(ctx, "gb_features_create(%d) -> %s", capacity, cudaGetErrorString(cudaGetLastError()));
+    rc = GB_ERR_CUDA;
+  }
+  if (rc != GB_OK) {
     gb_features_destroy(ctx, f);
-    return GB_ERR_CUDA;
+    return rc;
   }
   f->d_status = f->d_count + 1;
   f->d_train_status = f->d_count + 2;
@@ -302,12 +320,7 @@ int gb_features_destroy(gb_ctx* ctx, gb_features* f) {
     CtxLock lk(ctx);
     cudaStreamSynchronize(ctx->stream);
   }
-  cudaFree(f->d_kps);
-  cudaFree(f->d_desc);
-  cudaFree(f->d_count);
-  cudaFree(f->d_best);
-  cudaFree(f->d_dist);
-  cudaFree(f->d_dist2);
+  cudaFree(f->d_slab);
   delete f;
   return GB_OK;
 }

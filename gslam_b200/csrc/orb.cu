@@ -654,9 +654,9 @@ struct OrbState {
   gb_orb_cfg cfg{};
   OrbParams P{};
   FastMaps maps{};                      // TMA tensor maps of the pyramid levels (built with the buffers)
-  // device buffers
+  // device buffers: one allocation
+  void* d_slab = nullptr;
   uint8_t* d_pyr = nullptr; size_t pyr_bytes = 0;
-  void* d_color = nullptr; size_t color_cap = 0;  // packed colour frame before the gray conversion (grow-only)
   uint32_t* d_tabs = nullptr;           // resize tables
   uint32_t* d_cand_pos = nullptr; uint8_t* d_cand_score = nullptr; uint32_t* d_cand_key = nullptr; float* d_cand_resp = nullptr;
   uint32_t* d_surv_pos = nullptr;       // compact survivor lists share d_cand_key / d_cand_resp
@@ -667,20 +667,9 @@ struct OrbState {
   bool valid = false;
 };
 
-static void orb_free_buffers(OrbState* s) {
-  cudaFree(s->d_surv_pos); s->d_surv_pos = nullptr;
-  cudaFree(s->d_color); s->d_color = nullptr; s->color_cap = 0;
-  cudaFree(s->d_pyr); cudaFree(s->d_tabs); cudaFree(s->d_cand_pos); cudaFree(s->d_cand_score); cudaFree(s->d_cand_key);
-  cudaFree(s->d_cand_resp); cudaFree(s->d_counts); cudaFree(s->d_kept_pos); cudaFree(s->d_kept_resp);
-  s->d_pyr = nullptr; s->d_tabs = nullptr; s->d_cand_pos = nullptr; s->d_cand_score = nullptr; s->d_cand_key = nullptr;
-  s->d_cand_resp = nullptr; s->d_counts = nullptr; s->d_kept_pos = nullptr; s->d_kept_resp = nullptr;
-  s->valid = false;
-}
-
 void gb_orb_state_free(gb_ctx* ctx) {
   if (!ctx->orb) return;
-  orb_free_buffers(ctx->orb);
-  cudaFree(ctx->orb->d_pattern);
+  cudaFree(ctx->orb->d_slab);
   delete ctx->orb;
   ctx->orb = nullptr;
 }
@@ -704,22 +693,15 @@ static int orb_cfg_check(gb_ctx* ctx, const gb_orb_cfg* c) {
   return GB_OK;
 }
 
-static int orb_state_create(gb_ctx* ctx) {
-  if (ctx->orb) return GB_OK;
-  ctx->orb = new OrbState();
-  GB_CUDA(ctx, cudaMalloc((void**)&ctx->orb->d_pattern, 1024));
-  GB_CUDA(ctx, cudaMemcpyAsync(ctx->orb->d_pattern, kOrbPattern, 1024, cudaMemcpyHostToDevice, ctx->stream));
-  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return GB_OK;
-}
-
 // (Re)build the per-resolution state: level geometry, quotas, resize tables, buffers.
 static int orb_prepare(gb_ctx* ctx, int w, int h, const gb_orb_cfg* cfg) {
-  GB_CHECK(orb_state_create(ctx));
+  if (!ctx->orb) ctx->orb = new OrbState();
   OrbState* s = ctx->orb;
   if (s->valid && s->w == w && s->h == h && memcmp(&s->cfg, cfg, sizeof *cfg) == 0) return GB_OK;
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  orb_free_buffers(s);
+  cudaFree(s->d_slab);
+  s->d_slab = nullptr;
+  s->valid = false;
   if (w > 16384 || h > 16384) {
     gb_set_error(ctx, "gb_orb: image %dx%d too large (max 16384)", w, h);
     return GB_ERR_INVALID;
@@ -787,19 +769,19 @@ static int orb_prepare(gb_ctx* ctx, int w, int h, const gb_orb_cfg* cfg) {
     fill(S.w, D.w, tabs.data() + D.coef_off);
     fill(S.h, D.h, tabs.data() + D.coef_off + D.w);
   }
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_pyr, s->pyr_bytes));
-  GB_CUDA(ctx, cudaMemsetAsync(s->d_pyr, 0, s->pyr_bytes, ctx->stream));
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_tabs, tabs.size() * 4));
-  GB_CUDA(ctx, cudaMemcpyAsync(s->d_tabs, tabs.data(), tabs.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
   const size_t nc = (size_t)std::max(cand, 1);
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_cand_pos, nc * 4));
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_cand_score, nc));
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_cand_key, nc * 4));
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_cand_resp, nc * 4));
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_counts, (3 * kMaxLevels + 8 + kMaxLevels * 256) * sizeof(int)));
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_surv_pos, nc * 4));
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_kept_pos, (size_t)kMaxLevels * kSelMax * 4));
-  GB_CUDA(ctx, cudaMalloc((void**)&s->d_kept_resp, (size_t)kMaxLevels * kSelMax * 4));
+  GB_CHECK(gb_slab_alloc(ctx, &s->d_slab, [&](Slab& sl) {
+    sl.take(&s->d_pyr, s->pyr_bytes);
+    sl.take(&s->d_tabs, tabs.size());
+    sl.take(&s->d_cand_pos, nc); sl.take(&s->d_cand_score, nc); sl.take(&s->d_cand_key, nc); sl.take(&s->d_cand_resp, nc);
+    sl.take(&s->d_counts, 3 * kMaxLevels + 8 + kMaxLevels * 256);
+    sl.take(&s->d_surv_pos, nc);
+    sl.take(&s->d_kept_pos, (size_t)kMaxLevels * kSelMax); sl.take(&s->d_kept_resp, (size_t)kMaxLevels * kSelMax);
+    sl.take(&s->d_pattern, 1024);
+  }));
+  GB_CUDA(ctx, cudaMemsetAsync(s->d_pyr, 0, s->pyr_bytes, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(s->d_tabs, tabs.data(), tabs.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(s->d_pattern, kOrbPattern, 1024, cudaMemcpyHostToDevice, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // tabs is a local vector
   {  // TMA tensor maps: one per level over the padded-pitch buffer, u8, box = the FAST input tile; out-of-image reads give 0
     typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -879,24 +861,6 @@ static int orb_launch(gb_ctx* ctx, gb_features* out) {
   return GB_OK;
 }
 
-// Copy a frame into the dense frame buffer of the ctx's ORB state (d_color).
-static int orb_stage_copy(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row, int height, int pitch) {
-  OrbState* s = ctx->orb;
-  GB_CHECK(gb_dev_realloc(ctx, &s->d_color, &s->color_cap, row * height));
-  return gb_upload_2d(ctx, s->d_color, row, img, img_is_device, pitch, row, height);
-}
-
-int gb_orb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row_bytes, int height, int pitch, const uint8_t** d_frame) {
-  if (img_is_device && (size_t)pitch == row_bytes) {
-    *d_frame = img;
-    return GB_OK;
-  }
-  GB_CHECK(orb_state_create(ctx));
-  GB_CHECK(orb_stage_copy(ctx, img, img_is_device, row_bytes, height, pitch));
-  *d_frame = (const uint8_t*)ctx->orb->d_color;
-  return GB_OK;
-}
-
 extern "C" {
 
 void gb_orb_cfg_default(gb_orb_cfg* c) {
@@ -927,9 +891,9 @@ static int orb_extract_to_impl(gb_ctx* ctx, const uint8_t* img, int img_is_devic
   OrbState* s = ctx->orb;
   const LevelInfo& L0 = s->P.lv[0];
   if (channels != 1) {
-    GB_CHECK(orb_stage_copy(ctx, img, img_is_device, (size_t)width * channels, height, pitch));
-    orb_gray_kernel<<<dim3(gb_div_up(width, 256), height), 256, 0, ctx->stream>>>((const uint8_t*)s->d_color, width, height, channels, rgb_order,
-                                                                                 s->d_pyr + L0.off, L0.pitch);
+    const uint8_t* d_frame = nullptr;
+    GB_CHECK(gb_stage_frame(ctx, img, img_is_device, (size_t)width * channels, height, pitch, &d_frame));
+    orb_gray_kernel<<<dim3(gb_div_up(width, 256), height), 256, 0, ctx->stream>>>(d_frame, width, height, channels, rgb_order, s->d_pyr + L0.off, L0.pitch);
     GB_LAUNCH_CHECK(ctx);
   } else {
     GB_CHECK(gb_upload_2d(ctx, s->d_pyr + L0.off, L0.pitch, img, img_is_device, pitch, width, height));
@@ -969,7 +933,7 @@ static int orb_extract_undistorted_impl(gb_ctx* ctx, gb_remap* map, const uint8_
   GB_CHECK(orb_cfg_check(ctx, &cfg));
   GB_CHECK(orb_prepare(ctx, w_out, h_out, &cfg));
   const uint8_t* d_frame = nullptr;
-  GB_CHECK(gb_orb_stage_frame(ctx, img, img_is_device, (size_t)w_in * channels, h_in, pitch, &d_frame));
+  GB_CHECK(gb_stage_frame(ctx, img, img_is_device, (size_t)w_in * channels, h_in, pitch, &d_frame));
   OrbState* s = ctx->orb;
   const LevelInfo& L0 = s->P.lv[0];
   GB_CHECK(gb_remap_enqueue_level0(ctx, map, d_frame, channels, rgb_order, s->d_pyr + L0.off, L0.pitch));

@@ -304,20 +304,14 @@ int replay_stopping_rule(int n, int H, double confidence, const int* cnt, const 
 }
 
 // Uploads the correspondences, runs every hypothesis of gb_pnp_ransac on the device and brings back the per-hypothesis counts and
-// roots (pinned staging of this call); the winners' poses stay on the device at *d_Rt (rows of hypotheses with root -1 unwritten).
+// roots (pinned staging of this call); the winners' poses stay in the ctx's device scratch at *d_Rt (rows of hypotheses with root -1
+// unwritten).
 int pnp_run_hypotheses(gb_ctx* ctx, int n, const double* xyz, const double* xy, double thr2, uint64_t seed, int H, int** h_cnt_out,
                        int** h_root_out, double** d_Rt_out) {
-  // device buffers: points, measurements, per-hypothesis results (grow-only scratch owned by the ctx)
   const size_t b_xyz = (size_t)n * 24, b_xy = (size_t)n * 16, b_cnt = (size_t)H * 4, b_Rt = (size_t)H * 96;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t need = al(b_xyz) + al(b_xy) + 2 * al(b_cnt) + al(b_Rt);
-  GB_CHECK(gb_dev_realloc(ctx, &ctx->pnp_scratch, &ctx->pnp_scratch_cap, need));
-  uint8_t* base = (uint8_t*)ctx->pnp_scratch;
-  double* d_xyz = (double*)base; base += al(b_xyz);
-  double* d_xy = (double*)base; base += al(b_xy);
-  int* d_cnt = (int*)base; base += al(b_cnt);
-  int* d_root = (int*)base; base += al(b_cnt);
-  double* d_Rt = (double*)base;
+  double *d_xyz, *d_xy, *d_Rt;
+  int *d_cnt, *d_root;
+  GB_CHECK(gb_scratch_take(ctx, {{&d_xyz, b_xyz}, {&d_xy, b_xy}, {&d_cnt, b_cnt}, {&d_root, b_cnt}, {&d_Rt, b_Rt}}));
   double *h_xyz, *h_xy;
   int *h_cnt, *h_root;
   GB_CHECK(gb_stage_take(ctx, {{&h_xyz, b_xyz}, {&h_xy, b_xy}, {&h_cnt, b_cnt}, {&h_root, b_cnt}}));
@@ -465,26 +459,18 @@ GB_API int gb_dbg_pnp_hypotheses_host(int n, const double* xyz, const double* xy
 GB_API int gb_dbg_pnp_p3p_device(gb_ctx* ctx, int m, const double* X, const double* f, int* ns, double* Rt) {
   if (!ctx || m < 1 || !X || !f || !ns || !Rt) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  double *d_X = nullptr, *d_f = nullptr, *d_Rt = nullptr;
-  int* d_ns = nullptr;
-  int rc = GB_OK;
-  if (cudaMalloc(&d_X, (size_t)m * 72) != cudaSuccess || cudaMalloc(&d_f, (size_t)m * 72) != cudaSuccess ||
-      cudaMalloc(&d_Rt, (size_t)m * 384) != cudaSuccess || cudaMalloc(&d_ns, (size_t)m * 4) != cudaSuccess) {
-    gb_set_error(ctx, "gb_dbg_pnp_p3p_device: out of device memory");
-    rc = GB_ERR_CUDA;
-  } else {
-    cudaMemcpyAsync(d_X, X, (size_t)m * 72, cudaMemcpyHostToDevice, ctx->stream);
-    cudaMemcpyAsync(d_f, f, (size_t)m * 72, cudaMemcpyHostToDevice, ctx->stream);
-    cudaMemsetAsync(d_Rt, 0, (size_t)m * 384, ctx->stream);
-    pnp_p3p_kernel<<<gb_div_up(m, 128), 128, 0, ctx->stream>>>(m, d_X, d_f, d_ns, d_Rt);
-    ctx->launches++;
-    cudaMemcpyAsync(ns, d_ns, (size_t)m * 4, cudaMemcpyDeviceToHost, ctx->stream);
-    cudaMemcpyAsync(Rt, d_Rt, (size_t)m * 384, cudaMemcpyDeviceToHost, ctx->stream);
-    const cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { gb_set_error(ctx, "gb_dbg_pnp_p3p_device -> %s", cudaGetErrorString(e)); rc = GB_ERR_CUDA; }
-  }
-  cudaFree(d_X); cudaFree(d_f); cudaFree(d_Rt); cudaFree(d_ns);
-  return rc;
+  double *d_X, *d_f, *d_Rt;
+  int* d_ns;
+  GB_CHECK(gb_scratch_take(ctx, {{&d_X, (size_t)m * 72}, {&d_f, (size_t)m * 72}, {&d_Rt, (size_t)m * 384}, {&d_ns, (size_t)m * 4}}));
+  GB_CUDA(ctx, cudaMemcpyAsync(d_X, X, (size_t)m * 72, cudaMemcpyHostToDevice, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(d_f, f, (size_t)m * 72, cudaMemcpyHostToDevice, ctx->stream));
+  GB_CUDA(ctx, cudaMemsetAsync(d_Rt, 0, (size_t)m * 384, ctx->stream));
+  pnp_p3p_kernel<<<gb_div_up(m, 128), 128, 0, ctx->stream>>>(m, d_X, d_f, d_ns, d_Rt);
+  GB_LAUNCH_CHECK(ctx);
+  GB_CUDA(ctx, cudaMemcpyAsync(ns, d_ns, (size_t)m * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(Rt, d_Rt, (size_t)m * 384, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return GB_OK;
 }
 
 // every hypothesis of gb_pnp_ransac's minimal stage, launched exactly as gb_pnp_ransac launches it: cnt[H], root[H], Rt[12H]

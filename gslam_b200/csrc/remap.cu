@@ -15,15 +15,13 @@
 // writes the undistorted GRAY image straight into level 0 of the ORB pyramid, the colour conversion done in registers.
 #include "common.cuh"
 
-struct gb_remap {
+struct gb_remap {  // immutable after creation
   int device = 0;             // the table lives there: usable from every ctx on that device
   int w_in = 0, h_in = 0, w_out = 0, h_out = 0;
+  void* d_slab = nullptr;     // one allocation holding the three arrays below
   int32_t* d_idx = nullptr;   // [w_out*h_out][4]
   float* d_coef = nullptr;    // [w_out*h_out][4]
   float* d_x = nullptr;       // [w_out*h_out] remapX
-  uint8_t* d_src = nullptr;   // staging of the frame (grow-only); gb_remap_apply only
-  uint8_t* d_dst = nullptr;
-  size_t src_cap = 0, dst_cap = 0;
 };
 
 namespace {
@@ -131,17 +129,19 @@ int gb_remap_create(gb_ctx* ctx, int w_in, int h_in, int w_out, int h_out, const
   gb_remap* m = new gb_remap();
   m->device = ctx->device;
   m->w_in = w_in; m->h_in = h_in; m->w_out = w_out; m->h_out = h_out;
-  cudaError_t e = cudaMalloc((void**)&m->d_idx, n * 16);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&m->d_coef, n * 16);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&m->d_x, n * 4);
-  if (e == cudaSuccess) e = cudaMemcpy(m->d_idx, idx4, n * 16, cudaMemcpyHostToDevice);
+  int rc = gb_slab_alloc(ctx, &m->d_slab, [&](Slab& sl) { sl.take(&m->d_idx, 4 * n); sl.take(&m->d_coef, 4 * n); sl.take(&m->d_x, n); });
+  cudaError_t e = cudaSuccess;
+  if (rc == GB_OK) e = cudaMemcpy(m->d_idx, idx4, n * 16, cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(m->d_coef, coef4, n * 16, cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(m->d_x, remap_x, n * 4, cudaMemcpyHostToDevice);
   if (e != cudaSuccess) {
     gb_set_error(ctx, "gb_remap_create -> %s", cudaGetErrorString(e));
-    cudaFree(m->d_idx); cudaFree(m->d_coef); cudaFree(m->d_x);
+    rc = GB_ERR_CUDA;
+  }
+  if (rc != GB_OK) {
+    cudaFree(m->d_slab);
     delete m;
-    return GB_ERR_CUDA;
+    return rc;
   }
   *out = m;
   return GB_OK;
@@ -150,7 +150,7 @@ int gb_remap_create(gb_ctx* ctx, int w_in, int h_in, int w_out, int h_out, const
 int gb_remap_destroy(gb_ctx* ctx, gb_remap* m) {
   if (!m) return GB_OK;
   if (ctx) { CtxLock lk(ctx); cudaStreamSynchronize(ctx->stream); }
-  cudaFree(m->d_idx); cudaFree(m->d_coef); cudaFree(m->d_x); cudaFree(m->d_src); cudaFree(m->d_dst);
+  cudaFree(m->d_slab);
   delete m;
   return GB_OK;
 }
@@ -159,16 +159,14 @@ int gb_remap_apply(gb_ctx* ctx, gb_remap* m, const uint8_t* src, int channels, u
   if (!ctx || !m || !src || !dst || (channels != 1 && channels != 3)) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   const size_t n_in = (size_t)m->w_in * m->h_in, n_out = (size_t)m->w_out * m->h_out, b_in = n_in * channels, b_out = n_out * channels;
-  GB_CHECK(gb_dev_realloc(ctx, (void**)&m->d_src, &m->src_cap, b_in));
-  GB_CHECK(gb_dev_realloc(ctx, (void**)&m->d_dst, &m->dst_cap, b_out));
-  uint8_t *hs, *hd;
-  GB_CHECK(gb_stage_take(ctx, {{&hs, b_in}, {&hd, b_out}}));
-  memcpy(hs, src, b_in);
-  GB_CUDA(ctx, cudaMemcpyAsync(m->d_src, hs, b_in, cudaMemcpyHostToDevice, ctx->stream));
+  uint8_t *d_src, *d_dst, *hd;
+  GB_CHECK(gb_scratch_take(ctx, {{&d_src, b_in}, {&d_dst, b_out}}));
+  GB_CHECK(gb_upload_2d(ctx, d_src, b_in, src, 0, b_in, b_in, 1));
   remap_kernel<<<gb_div_up((int)n_out, 256), 256, 0, ctx->stream>>>((const int4*)m->d_idx, (const float4*)m->d_coef, m->d_x, (int)n_out, (int)n_in, channels,
-                                                                   m->d_src, m->d_dst, m->w_out, m->w_out * channels);
+                                                                   d_src, d_dst, m->w_out, m->w_out * channels);
   GB_LAUNCH_CHECK(ctx);
-  GB_CUDA(ctx, cudaMemcpyAsync(hd, m->d_dst, b_out, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CHECK(gb_stage_take(ctx, {{&hd, b_out}}));  // (after the upload's own take: a growth here synchronises first)
+  GB_CUDA(ctx, cudaMemcpyAsync(hd, d_dst, b_out, cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   memcpy(dst, hd, b_out);
   return GB_OK;
@@ -190,7 +188,7 @@ int gb_remap_apply_to(gb_ctx* ctx, gb_remap* m, const uint8_t* src, int src_is_d
     return GB_ERR_INVALID;
   }
   const uint8_t* d_src = nullptr;
-  GB_CHECK(gb_orb_stage_frame(ctx, src, src_is_device, (size_t)m->w_in * channels, m->h_in, src_pitch, &d_src));
+  GB_CHECK(gb_stage_frame(ctx, src, src_is_device, (size_t)m->w_in * channels, m->h_in, src_pitch, &d_src));
   const int n_out = m->w_out * m->h_out;
   remap_kernel<<<gb_div_up(n_out, 256), 256, 0, ctx->stream>>>((const int4*)m->d_idx, (const float4*)m->d_coef, m->d_x, n_out, m->w_in * m->h_in, channels, d_src,
                                                                 d_dst, m->w_out, dst_pitch);

@@ -187,10 +187,10 @@ GB_API int gb_remap_create(gb_ctx* ctx, int w_in, int h_in, int w_out, int h_out
                            const float* remap_x, gb_remap** out);
 GB_API int gb_remap_destroy(gb_ctx* ctx, gb_remap* map);
 GB_API int gb_remap_apply(gb_ctx* ctx, gb_remap* map, const uint8_t* src, int channels, uint8_t* dst);
-/* Device-resident forms.  gb_remap_apply keeps frame buffers inside the map, so a map is used by one gb_remap_apply at a time; the
- * three calls below only READ the map (whatever they stage lives in the ctx), so one map may serve any number of contexts on the
- * device it was created on, from any thread, at the same time.  A map of another device is GB_ERR_INVALID.  channels: 1 or 3 -- the
- * reference's 4-channel branch writes 3-channel pixels (Undistorter.h:336) and is not supported.
+/* Device-resident forms.  gb_remap_apply and the three calls below only READ the map (whatever they stage lives in the ctx), so one
+ * map may serve any number of contexts on the device it was created on, from any thread, at the same time.  A map of another device
+ * is GB_ERR_INVALID to the three calls below.  channels: 1 or 3 -- the reference's 4-channel branch writes 3-channel pixels
+ * (Undistorter.h:336) and is not supported.
  *
  * gb_remap_apply_to: undistort into device memory, enqueued on the ctx stream.  src: w_in x h_in pixels at src_pitch bytes per row
  * (>= w_in*channels), a device pointer (read in place when dense; no host synchronisation) or a host pointer (one synchronisation
@@ -221,7 +221,7 @@ GB_API int gb_orb_extract_undistorted(gb_ctx* ctx, gb_remap* map, const uint8_t*
  * ascending, feature indices ascending).  Word / node / feature indices are bit-exact with the reference; values are the reference's
  * floats, bit-exact for every vocabulary (accumulated with the same operations; the double L1 / L2 norm equals the reference's
  * sum in ascending word order).  One vocabulary may be used from any ctx on the device it was created on, from any thread: calls
- * on it are serialised by the vocabulary itself.  A leaf above level L - levelsup files under itself (the reference
+ * from different contexts run concurrently.  A leaf above level L - levelsup files under itself (the reference
  * reads an uninitialised node id there).  gb_bow_transform_features: the same for descriptors already resident in HBM (the output
  * of gb_orb_extract_to), no host round trip before the walk; the output arrays must hold the CAPACITY of `f` entries (the row
  * count of an extraction still in flight is only known on the device; the launch is clipped by it).  If that extraction failed

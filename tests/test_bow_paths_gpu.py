@@ -231,8 +231,9 @@ def test_transform_contracts(ctx):
 
 # ---- one vocabulary, two contexts, two threads -----------------------------------------------------------------------------------
 def test_one_vocabulary_two_contexts_two_threads(ctx):
-    """Two threads, each with its own ctx, transform their own descriptor sets through one vocabulary many times; every result
-    equals the oracle.  Both use the same row count, and one call at that count grew the vocabulary's scratch first."""
+    """Two threads, each with its own ctx, transform their own descriptor sets through one vocabulary many times, each set both from
+    host memory and as a device-resident feature set, so that host-buffer and device-feature transforms overlap; every result equals
+    the oracle.  Both use the same row count, and one call at that count ran first."""
     n, iters = 3000, 30
     v = O.synth_vocabulary(10, 4, seed=21, stop=0.05)
     dv = dev_voc(ctx, v)
@@ -240,16 +241,22 @@ def test_one_vocabulary_two_contexts_two_threads(ctx):
     sets = [[BC.queries(v, n, 100 * t + j) for j in range(2)] for t in range(2)]
     wants = [[O.bow_transform(v, s, 1) for s in ss] for ss in sets]
     ctxs = [ctx, Context(0)]
+    feats = [[Features(ctxs[t], n) for _ in range(2)] for t in range(2)]
+    for t in range(2):
+        for j in range(2):
+            feats[t][j].upload(sets[t][j])
     errors = []
 
     def run(t):
         try:
             for i in range(iters):
-                got = transform_on(ctxs[t], dv, sets[t][i % 2], 1, n)
-                for k in KEYS:
-                    if not np.array_equal(got[k], wants[t][i % 2][k]):
-                        errors.append((t, i, k))
-                        return
+                # thread 0 starts on host buffers, thread 1 on device features: the two forms run side by side
+                for src in ((sets, feats) if (i + t) % 2 == 0 else (feats, sets)):
+                    got = transform_on(ctxs[t], dv, src[t][i % 2], 1, n)
+                    for k in KEYS:
+                        if not np.array_equal(got[k], wants[t][i % 2][k]):
+                            errors.append((t, i, k, type(src[t][i % 2]).__name__))
+                            return
         except Exception as e:  # noqa: BLE001
             errors.append((t, repr(e)))
 
@@ -260,6 +267,8 @@ def test_one_vocabulary_two_contexts_two_threads(ctx):
         for x in th:
             x.join()
     finally:
+        for fs in feats[0] + feats[1]:
+            fs.close()
         dv.close()
         ctxs[1].close()
     assert not errors, errors

@@ -213,15 +213,17 @@ def test_one_map_serves_two_contexts_on_two_threads(ctx):
     kinds = ("gray", "bgr")
     want = [expected(size, k) for k in kinds]
     frames = [frame(size, k) for k in kinds]
+    want_und = [m.apply(f) for f in frames]  # gb_remap_apply from one thread: the map holds no per-call state
     ctxs = [Context(0), Context(0)]
     go = threading.Barrier(2)
-    got, err = [[], []], []
+    got, und, err = [[], []], [[], []], []
 
     def run(i):
         try:
             go.wait()
             for _ in range(4):
                 got[i].append(ctxs[i].orb_extract_undistorted(m, frames[i], n))
+                und[i].append(m.apply(frames[i], ctx=ctxs[i]))
         except BaseException as e:
             err.append(e)
             go.abort()
@@ -234,6 +236,8 @@ def test_one_map_serves_two_contexts_on_two_threads(ctx):
     for i in range(2):
         for kps, desc in got[i]:
             assert_features(kps, desc, want[i][0], want[i][1], kinds[i])
+        for u in und[i]:
+            assert np.array_equal(u, want_und[i]), kinds[i]
     for c in ctxs:
         c.close()
     m.close()
