@@ -15,8 +15,7 @@
 
 #include "../../include/gslam_b200.h"
 
-struct OrbState;    // orb.cu
-struct MatchState;  // match.cu
+struct OrbState;  // orb.cu
 
 // A grow-only buffer that one outermost API call on a ctx bump-allocates and CtxLock resets: the pinned staging, the device scratch.
 struct GbBump {
@@ -41,10 +40,7 @@ struct gb_ctx {
   int lock_depth = 0;
   // device state owned by subsystems
   OrbState* orb = nullptr;
-  MatchState* match = nullptr;
-  gb_features* tmp_q = nullptr;  // temporaries of the host-buffer match entry point
-  gb_features* tmp_t = nullptr;
-  gb_features* tmp_f = nullptr;  // temporary of the host-buffer extract entry point
+  int match_last_plan[4] = {0, 0, 0, 0};  // qtiles, nsplit, chunk, stereo of the last match launch (gb_dbg_match_last_plan); 0s: none
   void* ba_arena = nullptr;      // grow-only slab reused by the host-buffer BA entry points (no cudaMalloc per call)
   size_t ba_arena_cap = 0;
   bool ba_arena_busy = false;
@@ -61,6 +57,10 @@ struct gb_features {
   int* d_count = nullptr;        // device-side keypoint count (written by extract)
   int* d_status = nullptr;       // device-side status word (0 ok, else required capacity)
   int* d_train_status = nullptr; // status word of the train set of the last match with this set as query (written by the match)
+  // Split-merge tickets of the matches with this set as query, one per 128-row query tile, right after the four count words.
+  // Zero between launches: zeroed with the count words when the set is made, and the merging CTA of a tile re-arms its ticket.
+  // (Two contexts matching the same query set at once race on the tickets as they already do on d_best / d_dist / d_dist2.)
+  unsigned int* d_tickets = nullptr;
   int h_count = -1;              // host copy (valid when >=0)
   int expect = 0;                // expected row count while h_count is unknown (nfeatures of the extraction in flight): tunes launches
   int32_t* d_best = nullptr;     // match outputs [capacity]
@@ -88,14 +88,16 @@ struct GbBuf {
 // take of the same outermost call returned is dead.  Buffers that must be live at the same time are therefore taken in ONE call; a
 // nested call may take again only once its caller is done with its own earlier buffers.  GB_ERR_CUDA when the staging cannot grow.
 int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs);
-// The same for the ctx's grow-only device scratch: the per-call working memory of the host-buffer entry points, the staged frames and
-// the test hooks, so that the long-lived objects they read (maps, vocabularies) stay immutable after creation.  Two rules:
+// The same for the ctx's grow-only device scratch: the per-call working memory of the host-buffer entry points (their temporary feature
+// sets among it), the matcher's split partials, the staged frames and the test hooks, so that the long-lived objects they read (maps,
+// vocabularies) stay immutable after creation.  Two rules:
 //  * Take together.  Buffers that must be live at the same time are taken in one call: growing the scratch synchronises the stream
 //    and frees the old buffer, which kills every earlier take of the outermost call (bow_run takes the uploaded descriptors of
-//    gb_bow_transform with its word, key and output buffers).
+//    gb_bow_transform with its word, key and output buffers; gb_match_hamming its two feature sets with the partials).
 //  * No scratch access before gb_pdl_wait().  The next call on the ctx reuses the same bytes, ordered behind this call's kernels only
 //    by the stream, so a kernel launched with programmatic dependent launch must not read or write scratch before that wait
-//    (remap_level0_kernel reads only the map's table before it; every other kernel given scratch is a plain launch).
+//    (remap_level0_kernel reads only the map's table before it, match_kernel touches nothing before it; every other kernel given
+//    scratch is a plain launch).  And since the wait covers only the kernel's predecessor, every PDL kernel waits on every path.
 int gb_scratch_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs);
 // Enqueues the copy of `rows` rows of `row_bytes` from src (pitch spitch) to device memory d_dst (pitch dpitch) on the ctx stream:
 // device to device, pinned host memory directly, pageable host memory row by row through the pinned staging (one take).
@@ -103,7 +105,6 @@ int gb_upload_2d(gb_ctx* ctx, void* d_dst, size_t dpitch, const void* src, int s
 // A dense device copy of a frame (`height` rows of `row_bytes`): the frame itself when it is a device pointer with pitch == row_bytes,
 // else a copy in the ctx's device scratch (one take, then gb_upload_2d).
 int gb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t row_bytes, int height, int pitch, const uint8_t** d_frame);
-int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes);  // grow-only device buffer
 
 // ---- undistortion in front of the ORB extraction: what orb.cu needs of remap.cu ------------------------------------------------------
 void gb_remap_geometry(const gb_remap* m, int* device, int* w_in, int* h_in, int* w_out, int* h_out);
@@ -181,6 +182,24 @@ int gb_slab_alloc(gb_ctx* ctx, void** base, F&& layout) {
   layout(sl);
   return GB_OK;
 }
+
+// The same in ONE take of the ctx's device scratch (gb_scratch_take, and its rules): for the working memory of one call.
+template <typename F>
+int gb_scratch_slab(gb_ctx* ctx, F&& layout) {
+  Slab sl;
+  layout(sl);
+  uint8_t* base;
+  GB_CHECK(gb_scratch_take(ctx, {{&base, sl.off}}));
+  sl = Slab{base};
+  layout(sl);
+  return GB_OK;
+}
+
+constexpr int kQPerCta = 128;  // match.cu: threads per CTA == query rows per CTA, one split-merge ticket per such query tile
+// The arrays of a feature set of f->capacity rows: gb_features_create's allocation, and the temporaries of the host-buffer entry
+// points in the scratch.  gb_features_words(capacity) words from d_count on are the four count words and the tickets.
+void gb_features_layout(Slab& sl, gb_features* f);
+static inline int gb_features_words(int capacity) { return 4 + (capacity + kQPerCta - 1) / kQPerCta; }
 
 // ---- programmatic dependent launch (sm_90+): a kernel launched with gb_launch_pdl may be scheduled while its predecessor on
 // the stream is still running; it must call gb_pdl_wait() before touching anything the predecessor wrote.  Calling

@@ -78,20 +78,6 @@ int gb_stage_frame(gb_ctx* ctx, const uint8_t* img, int img_is_device, size_t ro
   return GB_OK;
 }
 
-int gb_dev_realloc(gb_ctx* ctx, void** p, size_t* cap, size_t bytes) {
-  if (bytes <= *cap && *p) return GB_OK;
-  if (*p) {
-    GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-  }
-  size_t want = bytes + (bytes >> 3) + 256;
-  GB_CUDA(ctx, cudaMalloc(p, want));
-  *cap = want;
-  return GB_OK;
-}
-
 namespace {
 struct FuncSetup {
   bool smem_ok = false;
@@ -127,7 +113,6 @@ bool gb_func_setup(gb_ctx* ctx, const void* fn, int smem, bool* nonportable_clus
 
 extern void gb_orb_state_free(gb_ctx* ctx);
 extern void ba_cache_drop(gb_ctx* ctx);
-extern void gb_match_state_free(gb_ctx* ctx);
 
 extern "C" {
 
@@ -219,12 +204,8 @@ int gb_ctx_destroy(gb_ctx* ctx) {
   {
     CtxLock lk(ctx);
     cudaStreamSynchronize(ctx->stream);
-    if (ctx->tmp_q) gb_features_destroy(ctx, ctx->tmp_q);
-    if (ctx->tmp_t) gb_features_destroy(ctx, ctx->tmp_t);
-    if (ctx->tmp_f) gb_features_destroy(ctx, ctx->tmp_f);
     ba_cache_drop(ctx);
     gb_orb_state_free(ctx);
-    gb_match_state_free(ctx);
     if (ctx->stage.base) cudaFreeHost(ctx->stage.base);
     cudaFree(ctx->scratch.base);
     cudaFree(ctx->ba_arena);
@@ -290,16 +271,8 @@ int gb_features_create(gb_ctx* ctx, int capacity, gb_features** out) {
   CtxLock lk(ctx);
   gb_features* f = new gb_features();
   f->capacity = capacity;
-  const size_t cap = (size_t)capacity;
-  int rc = gb_slab_alloc(ctx, &f->d_slab, [&](Slab& sl) {
-    sl.take(&f->d_kps, cap);
-    sl.take(&f->d_desc, cap * 32);
-    sl.take(&f->d_count, 4);  // count, status, train status, (pad)
-    sl.take(&f->d_best, cap);
-    sl.take(&f->d_dist, cap);
-    sl.take(&f->d_dist2, cap);
-  });
-  if (rc == GB_OK && cudaMemsetAsync(f->d_count, 0, 4 * sizeof(int), ctx->stream) != cudaSuccess) {
+  int rc = gb_slab_alloc(ctx, &f->d_slab, [&](Slab& sl) { gb_features_layout(sl, f); });
+  if (rc == GB_OK && cudaMemsetAsync(f->d_count, 0, gb_features_words(capacity) * sizeof(int), ctx->stream) != cudaSuccess) {
     gb_set_error(ctx, "gb_features_create(%d) -> %s", capacity, cudaGetErrorString(cudaGetLastError()));
     rc = GB_ERR_CUDA;
   }
@@ -307,8 +280,6 @@ int gb_features_create(gb_ctx* ctx, int capacity, gb_features** out) {
     gb_features_destroy(ctx, f);
     return rc;
   }
-  f->d_status = f->d_count + 1;
-  f->d_train_status = f->d_count + 2;
   f->h_count = 0;
   *out = f;
   return GB_OK;
@@ -326,6 +297,20 @@ int gb_features_destroy(gb_ctx* ctx, gb_features* f) {
 }
 
 }  // extern "C"
+
+void gb_features_layout(Slab& sl, gb_features* f) {
+  const size_t cap = (size_t)f->capacity;
+  sl.take(&f->d_kps, cap);
+  sl.take(&f->d_desc, cap * 32);
+  sl.take(&f->d_count, gb_features_words(f->capacity));  // count, status, train status, (pad), tickets: after d_desc (gb_match_hamming)
+  sl.take(&f->d_best, cap);
+  sl.take(&f->d_dist, cap);
+  sl.take(&f->d_dist2, cap);
+  if (!sl.base) return;  // (measuring)
+  f->d_status = f->d_count + 1;
+  f->d_train_status = f->d_count + 2;
+  f->d_tickets = (unsigned int*)(f->d_count + 4);
+}
 
 int gb_features_resolve(gb_ctx* ctx, gb_features* f, const int* hc, int* n) {
   if (hc[1] < 0) {

@@ -13,8 +13,6 @@
 
 namespace {
 
-constexpr int kQPerCta = 128;  // threads per CTA == queries per CTA
-
 struct MatchPartial {
   int32_t d0, b0, d1;
 };
@@ -164,39 +162,18 @@ __global__ void __launch_bounds__(256) popc_peak_kernel(unsigned int* __restrict
 
 }  // namespace
 
-struct MatchState {
-  void* d_partial = nullptr;
-  size_t partial_cap = 0;
-  void* d_tickets = nullptr;
-  size_t tickets_cap = 0;
-  int last_plan[4] = {0, 0, 0, 0};  // qtiles, nsplit, chunk, stereo of the last launch (gb_dbg_match_last_plan); 0s: none launched
+// The work split of a match launch, planned on the host: query tiles, train splits, rows per split, and the bytes of the per-split
+// partials the launch takes from the scratch.  nq / nt: the rows the launch covers; eq / et: the counts it is tuned for (<= 0: unknown,
+// use nq / nt).  nq <= 0 plans no launch.
+struct MatchPlan {
+  int qtiles = 0, nsplit = 0, chunk = 0;
+  size_t partial_bytes = 0;
 };
 
-void gb_match_state_free(gb_ctx* ctx) {
-  if (!ctx->match) return;
-  cudaFree(ctx->match->d_partial);
-  cudaFree(ctx->match->d_tickets);
-  delete ctx->match;
-  ctx->match = nullptr;
-}
-
-// Enqueue the match of (d_q, nq) against (d_t, nt) on the ctx stream.  Outputs are device pointers (may be null).
-// nq / nt: row counts, or -- with d_nq / d_nt -- CAPACITIES the launch must cover while the real counts are read on the device; the
-// work split is then tuned for the expected counts eq / et (<= 0: unknown, use the capacities).  d_train_status: see match_kernel.
-int gb_match_launch(gb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t, int nt, int32_t* d_best, int32_t* d_dist,
-                    int32_t* d_dist2, const int* d_nq = nullptr, const int* d_nt = nullptr, const StereoArgs* stereo = nullptr, int eq = 0,
-                    int et = 0, int* d_train_status = nullptr) {
-  if (!ctx->match) ctx->match = new MatchState();
-  MatchState* ms = ctx->match;
-  if (nq <= 0) {  // no query rows: nothing to launch, but the download still has to see the train set's status
-    ms->last_plan[0] = ms->last_plan[1] = ms->last_plan[2] = 0;
-    ms->last_plan[3] = stereo != nullptr;
-    if (d_train_status)
-      GB_CUDA(ctx, d_nt ? cudaMemcpyAsync(d_train_status, d_nt + 1, sizeof(int), cudaMemcpyDeviceToDevice, ctx->stream)
-                        : cudaMemsetAsync(d_train_status, 0, sizeof(int), ctx->stream));
-    return GB_OK;
-  }
-  const int qtiles = gb_div_up(nq, kQPerCta);
+static MatchPlan match_plan(const gb_ctx* ctx, int nq, int nt, int eq, int et) {
+  MatchPlan p;
+  if (nq <= 0) return p;
+  p.qtiles = gb_div_up(nq, kQPerCta);
   if (eq <= 0 || eq > nq) eq = nq;
   if (et <= 0 || et > nt) et = nt;
   // split the train rows so that ~2 CTAs land on every SM; chunk is a multiple of 8 rows, at most 1024 rows (32 KB)
@@ -214,26 +191,64 @@ int gb_match_launch(gb_ctx* ctx, const uint8_t* d_q, int nq, const uint8_t* d_t,
     nsplit = 1;
     chunk = 8;
   }
-  GB_CHECK(gb_dev_realloc(ctx, &ms->d_partial, &ms->partial_cap, (size_t)nsplit * nq * sizeof(MatchPartial)));
-  if ((size_t)qtiles * sizeof(unsigned int) > ms->tickets_cap) {
-    GB_CHECK(gb_dev_realloc(ctx, &ms->d_tickets, &ms->tickets_cap, (size_t)qtiles * sizeof(unsigned int)));
-    GB_CUDA(ctx, cudaMemsetAsync(ms->d_tickets, 0, ms->tickets_cap, ctx->stream));
+  p.nsplit = nsplit;
+  p.chunk = chunk;
+  p.partial_bytes = (size_t)nsplit * nq * sizeof(MatchPartial);
+  return p;
+}
+
+// The rows a match launch covers of f: its count, or -- while an extraction is in flight -- its capacity, which the kernel clips to
+// the device-side count.
+static int match_rows(const gb_features* f) { return f->h_count >= 0 ? f->h_count : f->capacity; }
+
+// Enqueue the match of fq against ft, planned as p (for match_rows of both), on the ctx stream: the partials at `partial`, the tickets
+// of fq, the outputs into fq for gb_match_download.  While either extraction is in flight the train set's status word is copied next
+// to fq's count words (see match_kernel).
+static int match_enqueue(gb_ctx* ctx, const MatchPlan& p, MatchPartial* partial, gb_features* fq, gb_features* ft, const StereoArgs* stereo) {
+  const bool pending = fq->h_count < 0 || ft->h_count < 0;
+  const int* d_nq = fq->h_count >= 0 ? nullptr : fq->d_count;
+  const int* d_nt = ft->h_count >= 0 ? nullptr : ft->d_count;
+  int* d_train_status = pending ? fq->d_train_status : nullptr;
+  const int nq = match_rows(fq), nt = match_rows(ft);
+  fq->n_matched = pending ? -1 : nq;  // -1: resolved by gb_match_download
+  int* plan = ctx->match_last_plan;
+  plan[0] = p.qtiles;
+  plan[1] = p.nsplit;
+  plan[2] = p.chunk;
+  plan[3] = stereo != nullptr;
+  if (nq <= 0) {  // no query rows: nothing to launch, but the download still has to see the train set's status
+    if (d_train_status)
+      GB_CUDA(ctx, d_nt ? cudaMemcpyAsync(d_train_status, d_nt + 1, sizeof(int), cudaMemcpyDeviceToDevice, ctx->stream)
+                        : cudaMemsetAsync(d_train_status, 0, sizeof(int), ctx->stream));
+    return GB_OK;
   }
-  dim3 grid(qtiles, nsplit);
-  const size_t smem = (size_t)chunk * (stereo ? 40 : 32);
-  StereoArgs sa = {};
-  if (stereo) sa = *stereo;
-  ms->last_plan[0] = qtiles;
-  ms->last_plan[1] = nsplit;
-  ms->last_plan[2] = chunk;
-  ms->last_plan[3] = stereo != nullptr;
-  if (stereo)
-    GB_CUDA(ctx, gb_launch_pdl(match_kernel<true>, grid, dim3(kQPerCta), smem, ctx->stream, (const uint4*)d_q, nq, (const uint4*)d_t, nt > 0 ? nt : 0, chunk,
-                               (MatchPartial*)ms->d_partial, (unsigned int*)ms->d_tickets, d_best, d_dist, d_dist2, d_nq, d_nt, d_train_status, sa));
-  else
-    GB_CUDA(ctx, gb_launch_pdl(match_kernel<false>, grid, dim3(kQPerCta), smem, ctx->stream, (const uint4*)d_q, nq, (const uint4*)d_t, nt > 0 ? nt : 0, chunk,
-                               (MatchPartial*)ms->d_partial, (unsigned int*)ms->d_tickets, d_best, d_dist, d_dist2, d_nq, d_nt, d_train_status, sa));
+  const size_t smem = (size_t)p.chunk * (stereo ? 40 : 32);
+  const StereoArgs sa = stereo ? *stereo : StereoArgs{};
+  GB_CUDA(ctx, gb_launch_pdl(stereo ? match_kernel<true> : match_kernel<false>, dim3(p.qtiles, p.nsplit), dim3(kQPerCta), smem, ctx->stream,
+                             (const uint4*)fq->d_desc, nq, (const uint4*)ft->d_desc, nt > 0 ? nt : 0, p.chunk, partial, fq->d_tickets, fq->d_best,
+                             fq->d_dist, fq->d_dist2, d_nq, d_nt, d_train_status, sa));
   GB_LAUNCH_CHECK(ctx);
+  return GB_OK;
+}
+
+// The match of two feature sets that live past the call: plan, take the partials from the scratch, enqueue.  eq / et: see match_plan.
+static int match_sets(gb_ctx* ctx, gb_features* fq, gb_features* ft, int eq, int et, const StereoArgs* stereo) {
+  const MatchPlan p = match_plan(ctx, match_rows(fq), match_rows(ft), eq, et);
+  MatchPartial* partial;
+  GB_CHECK(gb_scratch_take(ctx, {{&partial, p.partial_bytes}}));
+  return match_enqueue(ctx, p, partial, fq, ft, stereo);
+}
+
+// The temporaries of the host-buffer entry points, of nq and nt rows, and the partials of plan p: ONE take of the scratch (a second
+// take could grow it and free the first).  The caller zeroes the query set's count words and tickets; the train set is never a query.
+static int match_temporaries(gb_ctx* ctx, const MatchPlan& p, gb_features* fq, int nq, gb_features* ft, int nt, MatchPartial** partial) {
+  fq->capacity = nq;
+  ft->capacity = nt;
+  GB_CHECK(gb_scratch_slab(ctx, [&](Slab& sl) {
+    gb_features_layout(sl, fq);
+    gb_features_layout(sl, ft);
+    sl.take(partial, p.partial_bytes / sizeof(MatchPartial));
+  }));
   return GB_OK;
 }
 
@@ -270,45 +285,24 @@ GB_API int gb_dbg_popc_peak(gb_ctx* ctx, double* popc_per_s) {
 GB_API int gb_dbg_match_last_plan(gb_ctx* ctx, int* out) {
   if (!ctx || !out) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  for (int i = 0; i < 4; ++i) out[i] = ctx->match ? ctx->match->last_plan[i] : 0;
+  for (int i = 0; i < 4; ++i) out[i] = ctx->match_last_plan[i];
   return GB_OK;
 }
 
 int gb_match_features(gb_ctx* ctx, gb_features* fq, gb_features* ft) {
   if (!ctx || !fq || !ft) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  if (fq->h_count < 0 || ft->h_count < 0) {
-    // an extraction is still in flight: no host round trip -- launch for the capacities, the kernel reads the device-side counts
-    fq->n_matched = -1;  // resolved by gb_match_download
-    return gb_match_launch(ctx, fq->d_desc, fq->h_count >= 0 ? fq->h_count : fq->capacity, ft->d_desc, ft->h_count >= 0 ? ft->h_count : ft->capacity,
-                           fq->d_best, fq->d_dist, fq->d_dist2, fq->h_count >= 0 ? nullptr : fq->d_count, ft->h_count >= 0 ? nullptr : ft->d_count,
-                           nullptr, fq->expect, ft->expect, fq->d_train_status);
-  }
-  const int nq = fq->h_count, nt = ft->h_count;
-  fq->n_matched = nq;
-  return gb_match_launch(ctx, fq->d_desc, nq, ft->d_desc, nt, fq->d_best, fq->d_dist, fq->d_dist2);
+  // while an extraction is in flight there is no host round trip: the launch is tuned for the counts it expects
+  const bool pending = fq->h_count < 0 || ft->h_count < 0;
+  return match_sets(ctx, fq, ft, pending ? fq->expect : 0, pending ? ft->expect : 0, nullptr);
 }
 
 // Rectified-stereo row-band match, device-resident: left = query, right = train; results with gb_match_download(left).
 int gb_match_stereo_features(gb_ctx* ctx, gb_features* left, gb_features* right, float band_rows, float min_disparity, float max_disparity) {
   if (!ctx || !left || !right || !(band_rows >= 0.f) || !(max_disparity >= min_disparity)) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  StereoArgs sa;
-  sa.qk = left->d_kps; sa.tk = right->d_kps; sa.band = band_rows; sa.min_disp = min_disparity; sa.max_disp = max_disparity;
-  const bool async = left->h_count < 0 || right->h_count < 0;
-  left->n_matched = async ? -1 : left->h_count;
-  return gb_match_launch(ctx, left->d_desc, left->h_count >= 0 ? left->h_count : left->capacity, right->d_desc,
-                         right->h_count >= 0 ? right->h_count : right->capacity, left->d_best, left->d_dist, left->d_dist2,
-                         left->h_count >= 0 ? nullptr : left->d_count, right->h_count >= 0 ? nullptr : right->d_count, &sa, left->expect, right->expect,
-                         async ? left->d_train_status : nullptr);
-}
-
-// a temporary feature set of the host-buffer entry points (ctx->tmp_q / tmp_t) that holds at least n rows
-static int match_tmp_ensure(gb_ctx* ctx, gb_features** f, int n) {
-  if (*f && (*f)->capacity >= n) return GB_OK;
-  if (*f) gb_features_destroy(ctx, *f);
-  *f = nullptr;
-  return gb_features_create(ctx, n + n / 4 + 64, f);
+  const StereoArgs sa = {left->d_kps, right->d_kps, band_rows, min_disparity, max_disparity};
+  return match_sets(ctx, left, right, left->expect, right->expect, &sa);
 }
 
 // Host-buffer variant (what the Svar module's match_stereo binds).
@@ -316,14 +310,19 @@ int gb_match_stereo(gb_ctx* ctx, const gb_keypoint* kps_left, const uint8_t* des
                     int nr, float band_rows, float min_disparity, float max_disparity, int32_t* best_idx, int32_t* best_dist, int32_t* second_dist) {
   if (!ctx || nl < 0 || nr < 0 || (nl > 0 && (!kps_left || !desc_left)) || (nr > 0 && (!kps_right || !desc_right))) return GB_ERR_INVALID;
   if (nl == 0) return GB_OK;
+  if (!(band_rows >= 0.f) || !(max_disparity >= min_disparity)) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  GB_CHECK(match_tmp_ensure(ctx, &ctx->tmp_q, nl));
-  GB_CHECK(match_tmp_ensure(ctx, &ctx->tmp_t, nr > 0 ? nr : 1));
-  GB_CHECK(gb_features_upload(ctx, ctx->tmp_q, kps_left, desc_left, nl));
-  GB_CHECK(gb_features_upload(ctx, ctx->tmp_t, nr > 0 ? kps_right : nullptr, nr > 0 ? desc_right : desc_left, nr));
-  GB_CHECK(gb_match_stereo_features(ctx, ctx->tmp_q, ctx->tmp_t, band_rows, min_disparity, max_disparity));
+  const MatchPlan p = match_plan(ctx, nl, nr, 0, 0);
+  gb_features fq, ft;
+  MatchPartial* partial;
+  GB_CHECK(match_temporaries(ctx, p, &fq, nl, &ft, nr, &partial));
+  GB_CUDA(ctx, cudaMemsetAsync(fq.d_count, 0, gb_features_words(nl) * sizeof(int), ctx->stream));  // (the uploads set only two words)
+  GB_CHECK(gb_features_upload(ctx, &fq, kps_left, desc_left, nl));
+  GB_CHECK(gb_features_upload(ctx, &ft, nr > 0 ? kps_right : nullptr, nr > 0 ? desc_right : desc_left, nr));
+  const StereoArgs sa = {fq.d_kps, ft.d_kps, band_rows, min_disparity, max_disparity};
+  GB_CHECK(match_enqueue(ctx, p, partial, &fq, &ft, &sa));
   int n = nl;
-  return gb_match_download(ctx, ctx->tmp_q, best_idx, best_dist, second_dist, &n);
+  return gb_match_download(ctx, &fq, best_idx, best_dist, second_dist, &n);
 }
 
 int gb_match_download(gb_ctx* ctx, gb_features* fq, int32_t* best_idx, int32_t* best_dist, int32_t* second_dist, int* n) {
@@ -376,24 +375,26 @@ int gb_match_hamming(gb_ctx* ctx, const uint8_t* query, int nq, const uint8_t* t
   if (!ctx || nq < 0 || nt < 0 || (nq > 0 && !query) || (nt > 0 && !train)) return GB_ERR_INVALID;
   if (nq == 0) return GB_OK;
   CtxLock lk(ctx);
-  GB_CHECK(match_tmp_ensure(ctx, &ctx->tmp_q, nq));
-  GB_CHECK(match_tmp_ensure(ctx, &ctx->tmp_t, nt > 0 ? nt : 1));
-  gb_features *fq = ctx->tmp_q, *ft = ctx->tmp_t;
-  const size_t bq = (size_t)nq * 32, bt = (size_t)nt * 32;
+  const MatchPlan p = match_plan(ctx, nq, nt, 0, 0);
+  gb_features fq, ft;
+  MatchPartial* partial;
+  GB_CHECK(match_temporaries(ctx, p, &fq, nq, &ft, nt, &partial));
+  // the query rows, then zeros to the end of the count words and tickets that follow them: one copy
+  const size_t bq = (const uint8_t*)(fq.d_count + gb_features_words(nq)) - fq.d_desc, bt = (size_t)nt * 32;
   uint8_t *hq, *ht;
   GB_CHECK(gb_stage_take(ctx, {{&hq, bq}, {&ht, bt}}));
-  memcpy(hq, query, bq);
-  GB_CUDA(ctx, cudaMemcpyAsync(fq->d_desc, hq, bq, cudaMemcpyHostToDevice, ctx->stream));
+  memcpy(hq, query, (size_t)nq * 32);
+  memset(hq + (size_t)nq * 32, 0, bq - (size_t)nq * 32);
+  GB_CUDA(ctx, cudaMemcpyAsync(fq.d_desc, hq, bq, cudaMemcpyHostToDevice, ctx->stream));
   if (nt > 0) {
     memcpy(ht, train, bt);
-    GB_CUDA(ctx, cudaMemcpyAsync(ft->d_desc, ht, bt, cudaMemcpyHostToDevice, ctx->stream));
+    GB_CUDA(ctx, cudaMemcpyAsync(ft.d_desc, ht, bt, cudaMemcpyHostToDevice, ctx->stream));
   }
-  fq->h_count = nq;
-  ft->h_count = nt;
-  fq->n_matched = nq;
-  GB_CHECK(gb_match_launch(ctx, fq->d_desc, nq, ft->d_desc, nt, fq->d_best, fq->d_dist, fq->d_dist2));
+  fq.h_count = nq;
+  ft.h_count = nt;
+  GB_CHECK(match_enqueue(ctx, p, partial, &fq, &ft, nullptr));
   int n = nq;
-  return gb_match_download(ctx, fq, best_idx, best_dist, second_dist, &n);
+  return gb_match_download(ctx, &fq, best_idx, best_dist, second_dist, &n);
 }
 
 }  // extern "C"

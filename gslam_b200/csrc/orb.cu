@@ -823,8 +823,14 @@ static int orb_prepare(gb_ctx* ctx, int w, int h, const gb_orb_cfg* cfg) {
   return GB_OK;
 }
 
-// Enqueue the whole extraction of the frame already sitting in level 0 of the pyramid buffer.
-static int orb_launch(gb_ctx* ctx, gb_features* out) {
+// Enqueue the whole extraction of the frame already sitting in level 0 of the pyramid buffer.  tmp_cap > 0: `out` is a temporary of
+// tmp_cap rows, laid out over the scratch here, after level 0 was written (growing the scratch synchronises first, so the staged frame
+// it frees has been read).
+static int orb_launch(gb_ctx* ctx, gb_features* out, int tmp_cap) {
+  if (tmp_cap > 0) {
+    out->capacity = tmp_cap;
+    GB_CHECK(gb_scratch_slab(ctx, [&](Slab& sl) { gb_features_layout(sl, out); }));
+  }
   OrbState* s = ctx->orb;
   const OrbParams& P = s->P;
   cudaStream_t st = ctx->stream;
@@ -881,7 +887,7 @@ void gb_orb_cfg_default(gb_orb_cfg* c) {
 // channels: 1 = gray (GImage 8UC1), 3 / 4 = packed colour (8UC3 / 8UC4), converted on the device; rgb_order: 0 = B,G,R[,A] (OpenCV,
 // GSLAM IMAGE_BGRA), 1 = R,G,B[,A].  `pitch` is in bytes (>= width * channels).
 static int orb_extract_to_impl(gb_ctx* ctx, const uint8_t* img, int img_is_device, int width, int height, int pitch, const gb_orb_cfg* cfg_in,
-                               gb_features* out, bool sync_after, int channels = 1, int rgb_order = 0) {
+                               gb_features* out, bool sync_after, int channels = 1, int rgb_order = 0, int tmp_cap = 0) {
   if (!ctx || !img || !out || width < 1 || height < 1 || (channels != 1 && channels != 3 && channels != 4) || pitch < width * channels) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   gb_orb_cfg cfg;
@@ -898,7 +904,7 @@ static int orb_extract_to_impl(gb_ctx* ctx, const uint8_t* img, int img_is_devic
   } else {
     GB_CHECK(gb_upload_2d(ctx, s->d_pyr + L0.off, L0.pitch, img, img_is_device, pitch, width, height));
   }
-  GB_CHECK(orb_launch(ctx, out));
+  GB_CHECK(orb_launch(ctx, out, tmp_cap));
   if (!img_is_device && sync_after) GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staging / caller buffer may be reused
   return GB_OK;
 }
@@ -911,7 +917,7 @@ int gb_orb_extract_to(gb_ctx* ctx, const uint8_t* img, int img_is_device, int wi
 // The same with the frame undistorted on the way into level 0: the state is prepared for the map's OUTPUT size, the (dense) source
 // is remapped, and converted to gray when it has 3 channels, by one kernel that writes level 0; then the usual chain.
 static int orb_extract_undistorted_impl(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int img_is_device, int pitch, int channels, int rgb_order,
-                                        const gb_orb_cfg* cfg_in, gb_features* out, bool sync_after) {
+                                        const gb_orb_cfg* cfg_in, gb_features* out, bool sync_after, int tmp_cap = 0) {
   if (!ctx || !map || !img || !out) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   int device, w_in, h_in, w_out, h_out;
@@ -937,7 +943,7 @@ static int orb_extract_undistorted_impl(gb_ctx* ctx, gb_remap* map, const uint8_
   OrbState* s = ctx->orb;
   const LevelInfo& L0 = s->P.lv[0];
   GB_CHECK(gb_remap_enqueue_level0(ctx, map, d_frame, channels, rgb_order, s->d_pyr + L0.off, L0.pitch));
-  GB_CHECK(orb_launch(ctx, out));
+  GB_CHECK(orb_launch(ctx, out, tmp_cap));
   if (!img_is_device && sync_after) GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staging / caller buffer may be reused
   return GB_OK;
 }
@@ -975,29 +981,24 @@ static int orb_extract_host(gb_ctx* ctx, gb_remap* map, const uint8_t* img, int 
   if (cfg_in) cfg = *cfg_in; else gb_orb_cfg_default(&cfg);
   GB_CHECK(orb_cfg_check(ctx, &cfg));
   const int want_cap = std::max(*n, 2 * cfg.nfeatures + 256);
-  if (!ctx->tmp_f || ctx->tmp_f->capacity < want_cap) {
-    if (ctx->tmp_f) gb_features_destroy(ctx, ctx->tmp_f);
-    ctx->tmp_f = nullptr;
-    GB_CHECK(gb_features_create(ctx, want_cap, &ctx->tmp_f));
-  }
-  gb_features* f = ctx->tmp_f;
+  gb_features f;  // a temporary over the scratch, laid out by orb_launch
   if (map) {
     int device, w_in, h_in, w_out, h_out;
     gb_remap_geometry(map, &device, &w_in, &h_in, &w_out, &h_out);
-    GB_CHECK(orb_extract_undistorted_impl(ctx, map, img, 0, w_in * channels, channels, rgb_order, &cfg, f, *n <= 0));
+    GB_CHECK(orb_extract_undistorted_impl(ctx, map, img, 0, w_in * channels, channels, rgb_order, &cfg, &f, *n <= 0, want_cap));
   } else {
-    GB_CHECK(orb_extract_to_impl(ctx, img, 0, width, height, width * channels, &cfg, f, *n <= 0, channels, rgb_order));
+    GB_CHECK(orb_extract_to_impl(ctx, img, 0, width, height, width * channels, &cfg, &f, *n <= 0, channels, rgb_order, want_cap));
   }
   const int cap = *n;
   if (cap > 0) {  // one synchronisation: the count travels with the rows
     int m = cap;
-    const int rc = gb_features_download(ctx, f, kps, desc, &m);
+    const int rc = gb_features_download(ctx, &f, kps, desc, &m);
     *n = m;
     if (rc == GB_ERR_CAPACITY && m > cap) gb_set_error(ctx, "gb_orb_extract: %d keypoints > caller capacity %d", m, cap);
     return rc;
   }
   int cnt = 0;
-  const int rc = gb_features_count(ctx, f, &cnt);
+  const int rc = gb_features_count(ctx, &f, &cnt);
   *n = cnt;
   if (rc != GB_OK) return rc;
   if (cnt > 0) {

@@ -1,14 +1,16 @@
 """A ctx's device scratch grows inside the call whose take no longer fits it (gb_scratch_take, csrc/ctx.cu): the stream is synchronised,
 the buffer replaced, and the call's buffers are laid out in the new one.  Each case runs a call on a ctx whose scratch earlier calls
-sized too small, and compares its outputs byte for byte with the same call on a fresh ctx."""
+sized too small, and compares its outputs byte for byte with the same call on a fresh ctx -- for the matcher with the work split it
+planned (gb_dbg_match_last_plan)."""
 import numpy as np
 import pytest
 
-from gslam_b200 import synth
-from gslam_b200.api import Context, Remap, Vocabulary
+from gslam_b200 import capi, synth
+from gslam_b200.api import Context, Features, Remap, Vocabulary
 from oracle import oracle as O
 
 import _bow_cases as BC
+from _match_cases import grid_keypoints
 
 pytestmark = pytest.mark.gpu
 
@@ -108,3 +110,93 @@ def test_pnp_ransac_scratch_grows():
         assert np.array_equal(g[0], w[0]) and np.array_equal(g[1], w[1])
         for f in ("hypotheses", "best_hypothesis", "best_root", "inliers_minimal", "inliers_refined"):
             assert getattr(g[2], f) == getattr(w[2], f), f
+
+
+def last_plan(ctx):
+    out = np.zeros(4, np.int32)
+    assert capi.lib().gb_dbg_match_last_plan(ctx.handle, capi.ptr(out)) == capi.GB_OK
+    return tuple(int(x) for x in out)
+
+
+def test_device_match_partials_grow_then_tickets_rearm():
+    """Features.match takes its split partials from the scratch.  A small pair, then a pending pair (an extraction in flight) whose
+    partials grow the scratch and whose query capacity, 4001, leaves the last query tile -- and its ticket -- 33 rows, then the small
+    pair again, on the tickets its first match re-armed."""
+    small = synth.random_descriptors(200, 1), synth.random_descriptors(300, 2)
+    big = synth.random_descriptors(4001, 3), synth.random_descriptors(6000, 4)
+
+    def run(ctx, which):
+        sets = {}
+
+        def pair(name):
+            if name not in sets:
+                q, t = small if name == "small" else big
+                fq, ft = Features(ctx, len(q)), Features(ctx, len(t))
+                fq.upload(q)
+                ft.upload(t)
+                sets[name] = fq, ft
+            return sets[name]
+        out = []
+        try:
+            for name in which:
+                fq, ft = pair(name)
+                if name == "big":  # device-side counts: the launch covers the capacities, the last tile holds 28 real rows
+                    for f, n in ((fq, 3996), (ft, 5990)):
+                        assert capi.lib().gb_dbg_features_set_pending(ctx.handle, f._h, n, 0, n - 100) == capi.GB_OK
+                fq.match(ft)
+                out.append((last_plan(ctx), fq.matches()))
+        finally:
+            for fq, ft in sets.values():
+                fq.close()
+                ft.close()
+        return out
+    got = fresh(lambda c: run(c, ("small", "big", "small")))
+    want = [fresh(lambda c: run(c, (name,)))[0] for name in ("small", "big", "small")]
+    assert got[1][0][0] == 32 and got[1][0][1] > 1 and got[0][0][1] > 1, (got[0][0], got[1][0])
+    for (gp, gm), (wp, wm) in zip(got, want):
+        assert gp == wp
+        assert_same(gm, wm)
+    assert np.array_equal(got[0][1][0], got[2][1][0])
+
+
+def test_host_match_hamming_then_larger():
+    """gb_match_hamming: its two feature sets and the partials are one take, larger than the earlier call's."""
+    calls = [(synth.random_descriptors(150, 5), synth.random_descriptors(700, 6)),
+             (synth.random_descriptors(3000, 7), synth.random_descriptors(9000, 8))]
+
+    def run(ctx, cs):
+        return [(ctx.match_hamming(q, t), last_plan(ctx)) for q, t in cs]
+    got = fresh(lambda c: run(c, calls))
+    for g, call in zip(got, calls):
+        w = fresh(lambda c: run(c, [call]))[0]
+        assert g[1] == w[1]
+        assert_same(g[0], w[0])
+
+
+def test_host_match_stereo_then_larger():
+    """gb_match_stereo: the same for the rectified-stereo matcher, whose feature sets carry the keypoints."""
+    rng = np.random.default_rng(11)
+    calls = [(grid_keypoints(rng, n), synth.random_descriptors(n, 20 + n), grid_keypoints(rng, m), synth.random_descriptors(m, 30 + m))
+             for n, m in ((120, 400), (2500, 7000))]
+
+    def run(ctx, cs):
+        return [(ctx.match_stereo(*c, band=1.0, min_disp=0.0, max_disp=20.0), last_plan(ctx)) for c in cs]
+    got = fresh(lambda c: run(c, calls))
+    for g, call in zip(got, calls):
+        w = fresh(lambda c: run(c, [call]))[0]
+        assert g[1] == w[1] and g[1][3] == 1
+        assert_same(g[0], w[0])
+
+
+def test_orb_extract_large_capacity_then_small():
+    """gb_orb_extract's feature set is sized to the call, max(capacity, 2 nfeatures + 256), not to the largest earlier call."""
+    img = synth.synth_frame(640, 480, seed=9)
+    c = Context(0)
+    try:
+        got_big = c.orb_extract(img, 500, capacity=40000)
+        got = c.orb_extract(img, 500, capacity=600)
+    finally:
+        c.close()
+    assert len(got[0]) > 400
+    assert_same(got_big, fresh(lambda f: f.orb_extract(img, 500, capacity=40000)))
+    assert_same(got, fresh(lambda f: f.orb_extract(img, 500, capacity=600)))
