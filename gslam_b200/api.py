@@ -474,7 +474,8 @@ class BAGraph:
         return dict(U=U, gc=gc, V=V, gp=gp, W=W, cost=float(cost[0]))
 
     def force_generic_pcg(self, mode=1):
-        """PCG dispatch override (test hook): 0 auto, 1 generic multi-kernel, 2 one-cluster DSMEM, 3 single-CTA block-sparse."""
+        """PCG dispatch override (test hook): 0 auto, 1 generic multi-kernel, 2 one-cluster DSMEM, 3 single-CTA block-sparse, 4 one-cluster
+        DSMEM in a cluster of 8 CTAs."""
         self.ctx._check(self.ctx._lib.gb_dbg_ba_force_generic_pcg(self.ctx._h, self._h, int(mode)))
 
     def set_cam_split(self, split: int):
@@ -493,6 +494,7 @@ class BAGraph:
 
     # bits of paths(): what a solve of this graph would run, as planned now (gb_dbg_ba_paths in csrc/ba.cu)
     LOCAL4, PCG_SPARSE, PCG_CLUSTER, PCG_BCSR, BCSR_CLUSTER, SCHUR_CHUNKS, SWEEP_LARGE, DENSE_ATOMIC, CHOL_OK, CAM_SPLIT = (1 << k for k in range(10))
+    SPARSE_SMALL, SPARSE_LONG_ROWS = 1 << 10, 1 << 11   # which single-CTA sparse PCG instantiation (set with PCG_SPARSE only)
 
     def paths(self) -> int:
         """Bitmask of the solver paths (test hook): see the BAGraph.LOCAL4 ... CAM_SPLIT constants."""
@@ -507,6 +509,17 @@ class BAGraph:
         o = (cfg or OptimzeConfig()).to_c()
         self.ctx._check(self.ctx._lib.gb_dbg_ba_reduced(self.ctx._h, self._h, C.byref(o), ptr(S), ptr(gt), ptr(dc), C.byref(it)))
         return S, gt, dc, it.value
+
+    def dbg_system(self, cfg: OptimzeConfig | None = None):
+        """The linear system of one LM step at the current estimate and the answer of the solver that step would run (test hook,
+        gb_dbg_ba_system): dict(S = undamped 6N x 6N, gt, diagU, lam, x, iters).  The damped system is S with, on its diagonal,
+        S_dd + lam * clamp(diagU_d, 1e-6, 1e32) at a free dof and 1 at a fixed one."""
+        n6 = 6 * self.n_cams
+        S = np.zeros((n6, n6)); gt = np.zeros(n6); dU = np.zeros(n6); x = np.zeros(n6); lam = C.c_double(); it = C.c_int()
+        o = (cfg or OptimzeConfig()).to_c()
+        self.ctx._check(self.ctx._lib.gb_dbg_ba_system(self.ctx._h, self._h, C.byref(o), ptr(S), ptr(gt), ptr(dU), C.byref(lam), ptr(x),
+                                                       C.byref(it)))
+        return dict(S=S, gt=gt, diagU=dU, lam=lam.value, x=x, iters=it.value)
 
 
 

@@ -1438,8 +1438,9 @@ static int ba_validate(gb_ctx* ctx, const gb_ba_problem* pb) {
   return GB_OK;
 }
 
-// Can the reduced camera system be solved by the one-cluster PCG kernel?  Pick the cluster size, remember the smem need.
-static void ba_pick_pcg(gb_ctx* ctx, gb_ba_graph* g) {
+// Can the reduced camera system be solved by the one-cluster PCG kernel?  Pick the cluster size (the largest of 16 and 8 that fits,
+// at most max_cluster), remember the smem need.
+static void ba_pick_pcg(gb_ctx* ctx, gb_ba_graph* g, int max_cluster = 16) {
   g->pcg_cluster = 0;
   g->pcg_sparse = false;
   const int nc = g->d.nc, n6 = g->d.n6;
@@ -1461,7 +1462,7 @@ static void ba_pick_pcg(gb_ctx* ctx, gb_ba_graph* g) {
   const int sizes[2] = {16, 8};
   for (int t = 0; t < 2; ++t) {
     const int C = sizes[t];
-    if (C == 16 && !np_ok) continue;
+    if ((C == 16 && !np_ok) || C > max_cluster) continue;
     const int cpc = (nc + C - 1) / C;
     const size_t smem = ((size_t)6 * cpc * n6 + (size_t)nc * 36 + 7 * (size_t)n6) * sizeof(double) + 64;
     if (smem + 2048 > (size_t)ctx->max_smem_optin || !smem_ok) continue;
@@ -2146,9 +2147,14 @@ extern "C" {
 // single-CTA block-sparse PCG, in the variant that fits the graph's active cameras and its longest block row of S (the
 // shared-memory path for columns beyond the registers is compiled in only where a row needs it; pdl: programmatic dependent
 // launch)
+static void ba_pcg_sparse_variant(const gb_ba_graph* g, bool* small, bool* long_rows) {
+  *small = g->pcg_nact <= kSpSmallCams;
+  *long_rows = 6 * g->pcg_max_row_blocks > 8 * (*small ? kSpSmallCols : kSpLargeCols);
+}
+
 static int ba_pcg_sparse_launch(gb_ctx* ctx, gb_ba_graph* g, double* buf, bool pdl) {
-  const bool small = g->pcg_nact <= kSpSmallCams;
-  const bool long_rows = 6 * g->pcg_max_row_blocks > 8 * (small ? kSpSmallCols : kSpLargeCols);
+  bool small, long_rows;
+  ba_pcg_sparse_variant(g, &small, &long_rows);
   void (*kernel)(BaDev, double*, int) = small ? (long_rows ? BA_SPARSE_SMALL(true) : BA_SPARSE_SMALL(false))
                                               : (long_rows ? BA_SPARSE_LARGE(true) : BA_SPARSE_LARGE(false));
   const dim3 block(small ? kSpSmallThreads : kSpLargeThreads);
@@ -2418,9 +2424,12 @@ static int ba_graph_refresh(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_problem* pb
 // the bits of gb_dbg_ba_paths (below)
 static int ba_paths(const gb_ba_graph* g) {
   const BaDev& d = g->d;
+  bool small, long_rows;
+  ba_pcg_sparse_variant(g, &small, &long_rows);
   return (ba_takes_local4(g) ? 1 : 0) | (g->pcg_sparse ? 2 : 0) | (g->pcg_cluster > 0 ? 4 : 0) | (g->pcg_bcsr ? 8 : 0) |
          (g->pcg_bcsr && g->bcsr_cluster > 0 ? 16 : 0) | (d.sp_nchunks > 0 ? 32 : 0) | (ba_sweep_is_large(g) ? 64 : 0) |
-         (d.s_nnzb == 0 && d.nc > 0 ? 128 : 0) | (g->chol_ok ? 256 : 0) | (d.cam_split > 1 ? 512 : 0);
+         (d.s_nnzb == 0 && d.nc > 0 ? 128 : 0) | (g->chol_ok ? 256 : 0) | (d.cam_split > 1 ? 512 : 0) |
+         (g->pcg_sparse && small ? 1024 : 0) | (g->pcg_sparse && long_rows ? 2048 : 0);
 }
 
 extern "C" int gb_ba_solve(gb_ctx* ctx, gb_ba_problem* pb, const gb_ba_options* opt, gb_ba_result* res) {
@@ -2551,15 +2560,62 @@ GB_API int gb_dbg_ba_reduced(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* o
   return GB_OK;
 }
 
+// The linear system one LM step of this graph would solve, and the answer of the solver that step would run: begin, the
+// reduction onto the layout a solve uses (the compact block-CSR one when the multi-CTA block-CSR PCG solves it), then that
+// solver alone -- single-CTA sparse, one-cluster, generic or block-CSR PCG, or the direct solver.  Out, each where non-null: S
+// (6N x 6N dense, UNDAMPED, read before the solver damps its copy), g~ and diag U (n6 each), lambda (the damped system is S with
+// lm_damp(S_dd, diagU_d, lambda) on its diagonal), the solution x (n6) and the PCG iterations (0 for the direct solver).
+GB_API int gb_dbg_ba_system(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt, double* S, double* gt, double* diagU,
+                            double* lambda, double* x, int* pcg_iters) {
+  if (!ctx || !g) return GB_ERR_INVALID;
+  CtxLock lk(ctx);
+  GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
+  const BaDev& d = g->d;
+  const size_t n6 = d.n6, nnzb = d.s_nnzb;
+  const bool compact = !ba_takes_local4(g) && g->pcg_bcsr && g->opt.linear_solver == 0;
+  // where S is read from: the compact buffer, the block-CSR values (the single-CTA PCG and the direct solver read only those), or
+  // the dense layout (one-cluster / generic PCG, pose-graph coupling included)
+  const bool dense_S = !compact && !(nnzb > 0 && (g->pcg_sparse || g->opt.linear_solver == 1));
+  const double* blocks = compact ? g->rbuf : d.Sb;
+  const double* tail = compact ? g->rbuf + nnzb * 36 : g->buf + n6 * n6;
+  if (compact) GB_CHECK(ba_compact_reduce(ctx, g, nullptr));
+  else GB_CHECK(gb_ba_graph_reduce_local(ctx, g, nullptr));
+  std::vector<double> sb(dense_S ? 0 : nnzb * 36);
+  std::vector<int> brow(dense_S ? 0 : nnzb), col(dense_S ? 0 : nnzb);
+  if (S && dense_S) GB_CUDA(ctx, cudaMemcpyAsync(S, g->buf, n6 * n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  if (S && !dense_S && nnzb > 0) {
+    GB_CUDA(ctx, cudaMemcpyAsync(sb.data(), blocks, nnzb * 36 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    GB_CUDA(ctx, cudaMemcpyAsync(brow.data(), d.s_brow, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    GB_CUDA(ctx, cudaMemcpyAsync(col.data(), d.s_col, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if (gt) GB_CUDA(ctx, cudaMemcpyAsync(gt, tail, n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  if (diagU) GB_CUDA(ctx, cudaMemcpyAsync(diagU, tail + n6, n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // (the solver below damps S in place on some paths)
+  if (compact) GB_CHECK(ba_pcg_bcsr_launch(ctx, g, g->rbuf));
+  else GB_CHECK(ba_pcg_dispatch(ctx, g, g->buf));
+  if (x) GB_CUDA(ctx, cudaMemcpyAsync(x, d.x, n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  BaScalars h;
+  GB_CHECK(ba_read_scalars(ctx, g, &h));
+  if (S && !dense_S) {
+    memset(S, 0, n6 * n6 * sizeof(double));
+    for (size_t blk = 0; blk < nnzb; ++blk)
+      for (int k = 0; k < 36; ++k) S[(6 * (size_t)brow[blk] + k / 6) * n6 + 6 * (size_t)col[blk] + k % 6] = sb[36 * blk + k];
+  }
+  if (lambda) *lambda = h.lambda;
+  if (pcg_iters) *pcg_iters = h.pcg_iters;
+  return GB_OK;
+}
+
 // force (1) / release (0) the generic multi-kernel PCG on this graph — lets the tests cover both solver paths
-// on: 0 = automatic dispatch, 1 = generic multi-kernel PCG, 2 = one-cluster DSMEM PCG (if it fits), 3 = single-CTA sparse
+// on: 0 = automatic dispatch, 1 = generic multi-kernel PCG, 2 = one-cluster DSMEM PCG (if it fits), 3 = single-CTA sparse,
+// 4 = one-cluster DSMEM PCG in a cluster of 8 CTAs (the size taken where 16-CTA clusters are not available)
 GB_API int gb_dbg_ba_force_generic_pcg(gb_ctx* ctx, gb_ba_graph* g, int on) {
   if (!ctx || !g) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  ba_pick_pcg(ctx, g);
+  ba_pick_pcg(ctx, g, on == 4 ? 8 : 16);
   if (g->d.npe > 0) g->pcg_sparse = false;  // (pose-graph terms live on the dense reduced system)
   if (on == 1) { g->pcg_cluster = 0; g->pcg_sparse = false; }
-  if (on == 2) g->pcg_sparse = false;
+  if (on == 2 || on == 4) g->pcg_sparse = false;
   if (on == 3) g->pcg_cluster = 0;
   return GB_OK;
 }
@@ -2601,6 +2657,8 @@ GB_API int gb_dbg_ba_pcg_cluster_size(gb_ctx* ctx, gb_ba_graph* g) { return (ctx
 //   8 pcg_bcsr: compact block-CSR PCG               16 ... in one thread-block cluster (else as a cooperative grid)
 //   32 landmark-chunk Schur plan (else block gather)   64 persistent large-graph sweep (ba_sweep.cu)
 //   128 no block structure: dense Schur by fp64 atomics   256 chol_ok: the direct solver fits   512 camera pass sliced (cam_split > 1)
+//   1024 ... the single-CTA sparse PCG in its 12-warp instantiation (<= kSpSmallCams active cameras; else the 20-warp one)
+//   2048 ... in its variant for block rows longer than the register columns (shared-memory mat-vec tail)
 // Tests assert these bits so that a threshold change cannot quietly turn one path's test into a duplicate of another's.
 GB_API int gb_dbg_ba_paths(gb_ctx* ctx, gb_ba_graph* g) { return (ctx && g) ? ba_paths(g) : -1; }
 
