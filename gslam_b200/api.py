@@ -495,6 +495,7 @@ class BAGraph:
     # bits of paths(): what a solve of this graph would run, as planned now (gb_dbg_ba_paths in csrc/ba.cu)
     LOCAL4, PCG_SPARSE, PCG_CLUSTER, PCG_BCSR, BCSR_CLUSTER, SCHUR_CHUNKS, SWEEP_LARGE, DENSE_ATOMIC, CHOL_OK, CAM_SPLIT = (1 << k for k in range(10))
     SPARSE_SMALL, SPARSE_LONG_ROWS = 1 << 10, 1 << 11   # which single-CTA sparse PCG instantiation (set with PCG_SPARSE only)
+    SCHUR_PASSES = 1 << 12                               # a Schur chunk uses more than 80 slots: the chunk kernel's second pass runs
 
     def paths(self) -> int:
         """Bitmask of the solver paths (test hook): see the BAGraph.LOCAL4 ... CAM_SPLIT constants."""
@@ -521,6 +522,12 @@ class BAGraph:
                                                        C.byref(it)))
         return dict(S=S, gt=gt, diagU=dU, lam=lam.value, x=x, iters=it.value)
 
+    def dbg_last_step(self):
+        """What the last LM iteration left on the device (test hook, gb_dbg_ba_last_step): dict(x = camera step (6N), vinv = damped
+        landmark inverses (np x 3 x 3), pts_new = candidate landmarks (np x 3))."""
+        x = np.zeros(6 * self.n_cams); vinv = np.zeros((self.n_points, 3, 3)); pn = np.zeros((self.n_points, 3))
+        self.ctx._check(self.ctx._lib.gb_dbg_ba_last_step(self.ctx._h, self._h, ptr(x), ptr(vinv), ptr(pn)))
+        return dict(x=x, vinv=vinv, pts_new=pn)
 
 
 class Comm:

@@ -135,6 +135,7 @@ _DEBUG_SIGNATURES = [
     ("gb_dbg_ba_linearize", C.c_int, [_VP, _VP, C.c_double, _VP, _VP, _VP, _VP, _VP, _VP]),
     ("gb_dbg_ba_reduced", C.c_int, [_VP, _VP, C.POINTER(BaOptions), _VP, _VP, _VP, C.POINTER(C.c_int)]),
     ("gb_dbg_ba_system", C.c_int, [_VP, _VP, C.POINTER(BaOptions), _VP, _VP, _VP, C.POINTER(C.c_double), _VP, C.POINTER(C.c_int)]),
+    ("gb_dbg_ba_last_step", C.c_int, [_VP, _VP, _VP, _VP, _VP]),
     ("gb_dbg_ba_force_generic_pcg", C.c_int, [_VP, _VP, C.c_int]),
     ("gb_dbg_ba_pcg_cluster_size", C.c_int, [_VP, _VP]),
     ("gb_dbg_ba_pcg_sparse", C.c_int, [_VP, _VP]),

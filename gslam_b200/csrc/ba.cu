@@ -1808,6 +1808,7 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
     ba_pcg_bcsr_plan(ctx, g, s_rowptr.data(), s_col.data(), bcsr_cta_cam);
     if (!getenv("GB_BA_NO_SCHUR_CHUNKS")) ba_schur_plan(ctx, g, np, pt_off, scam, pfree.data(), s_rowptr, s_col, s_upper, schur);  // (optional: the block-gather kernel otherwise)
   }
+  g->sp_max_nused = d.sp_nchunks > 0 ? *std::max_element(schur.nused.begin(), schur.nused.end()) : 0;
   if (compact_only && !g->pcg_bcsr) {
     gb_set_error(ctx, "gb_ba: the sharded solve needs the block-CSR reduced system (<= %d cameras)", kMaxBlockCams);
     return GB_ERR_INVALID;
@@ -2429,7 +2430,8 @@ static int ba_paths(const gb_ba_graph* g) {
   return (ba_takes_local4(g) ? 1 : 0) | (g->pcg_sparse ? 2 : 0) | (g->pcg_cluster > 0 ? 4 : 0) | (g->pcg_bcsr ? 8 : 0) |
          (g->pcg_bcsr && g->bcsr_cluster > 0 ? 16 : 0) | (d.sp_nchunks > 0 ? 32 : 0) | (ba_sweep_is_large(g) ? 64 : 0) |
          (d.s_nnzb == 0 && d.nc > 0 ? 128 : 0) | (g->chol_ok ? 256 : 0) | (d.cam_split > 1 ? 512 : 0) |
-         (g->pcg_sparse && small ? 1024 : 0) | (g->pcg_sparse && long_rows ? 2048 : 0);
+         (g->pcg_sparse && small ? 1024 : 0) | (g->pcg_sparse && long_rows ? 2048 : 0) |
+         (d.sp_nchunks > 0 && g->sp_max_nused > kChunkSlotsPerPass ? 4096 : 0);
 }
 
 extern "C" int gb_ba_solve(gb_ctx* ctx, gb_ba_problem* pb, const gb_ba_options* opt, gb_ba_result* res) {
@@ -2606,6 +2608,20 @@ GB_API int gb_dbg_ba_system(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* op
   return GB_OK;
 }
 
+// What the graph's last LM iteration left on the device, copied back without a launch, each where non-null: the camera step x (n6),
+// the damped landmark inverses V~^-1 (np x 9: at the lambda of that iteration, or at the new one after a rejection on the local-BA
+// chain, which refreshes them) and the candidate landmarks pts_new (np x 3).  Landmarks in the caller's order (of this shard).
+GB_API int gb_dbg_ba_last_step(gb_ctx* ctx, gb_ba_graph* g, double* x, double* vinv, double* pts_new) {
+  if (!ctx || !g) return GB_ERR_INVALID;
+  CtxLock lk(ctx);
+  const BaDev& d = g->d;
+  if (x && d.n6 > 0) GB_CUDA(ctx, cudaMemcpyAsync(x, d.x, (size_t)d.n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  if (vinv && d.np > 0) GB_CUDA(ctx, cudaMemcpyAsync(vinv, d.Vinv, (size_t)d.np * 9 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  if (pts_new && d.np > 0) GB_CUDA(ctx, cudaMemcpyAsync(pts_new, d.pts_new, (size_t)d.np * 3 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return GB_OK;
+}
+
 // force (1) / release (0) the generic multi-kernel PCG on this graph — lets the tests cover both solver paths
 // on: 0 = automatic dispatch, 1 = generic multi-kernel PCG, 2 = one-cluster DSMEM PCG (if it fits), 3 = single-CTA sparse,
 // 4 = one-cluster DSMEM PCG in a cluster of 8 CTAs (the size taken where 16-CTA clusters are not available)
@@ -2659,6 +2675,7 @@ GB_API int gb_dbg_ba_pcg_cluster_size(gb_ctx* ctx, gb_ba_graph* g) { return (ctx
 //   128 no block structure: dense Schur by fp64 atomics   256 chol_ok: the direct solver fits   512 camera pass sliced (cam_split > 1)
 //   1024 ... the single-CTA sparse PCG in its 12-warp instantiation (<= kSpSmallCams active cameras; else the 20-warp one)
 //   2048 ... in its variant for block rows longer than the register columns (shared-memory mat-vec tail)
+//   4096 a chunk of the landmark-chunk Schur plan uses more than 80 slots: ba_schur_chunks_kernel runs its second slot pass
 // Tests assert these bits so that a threshold change cannot quietly turn one path's test into a duplicate of another's.
 GB_API int gb_dbg_ba_paths(gb_ctx* ctx, gb_ba_graph* g) { return (ctx && g) ? ba_paths(g) : -1; }
 

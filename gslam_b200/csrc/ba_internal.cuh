@@ -43,6 +43,7 @@ struct gb_ba_graph {
   bool pcg_sparse = false;
   size_t pcg_sparse_smem = 0;
   int pcg_max_row_blocks = 0;  // longest block row of S
+  int sp_max_nused = 0;         // most slots any chunk of the landmark-chunk Schur plan uses (> 80: ba_schur_chunks_kernel runs a 2nd pass)
   int sweep_mode = 0;           // 0 = by size (ba_sweep.cu from 64k observations), 1 = ba.cu's latency-tuned kernel, 2 = ba_sweep.cu
   bool sweep_only = false;     // the last begin came from gb_ba_graph_sweep and nothing else ran since
   int pcg_nact = 0;            // cameras with at least one free dof (the sparse PCG kernel gives lanes to these only)

@@ -12,6 +12,8 @@ Each builder here starts from `synth_ba` and edits it into one named shape, dete
   two_components      two disconnected trajectories, each with its own fixed camera
   measurement_forms   obs_xyz with z != 1 (negative too), non-unit quaternions, non-symmetric information, a Huber delta that
                       residuals straddle, landmarks behind some of their observing cameras
+  long_tracks         free landmarks with exactly 13, 14, 15 and 16 observers (consecutive and scattered) and with 8 and 9: a Schur
+                      chunk over more than 12 cameras, worked in two slot passes
 
 `build(name, large)`: the small size is a local-BA window (<= 80 active cameras); the large one has more than 80 active cameras and
 more than 65 536 observations, so the compact path and the persistent sweep run by their own thresholds.
@@ -167,13 +169,119 @@ def measurement_forms(large: bool) -> Case:
     return Case("measurement_forms", pb, delta=float(np.quantile(e, 0.6)))
 
 
-CASES = {f.__name__: f for f in (scattered_fixed, isolated_cameras, sparse_landmarks, wide_landmarks, two_components, measurement_forms)}
+def long_tracks(large: bool) -> Case:
+    pb = _base(large, 108)
+    rng = np.random.default_rng(10)
+    nc = pb.n_cams
+    # 13..16 observers: the most a Schur chunk takes (16 cameras) and more than its one-pass 80 slots (12 cameras = 78 slots); on
+    # consecutive keyframes and scattered over a window with gaps (small: every block stays inside a 24-camera window, so S keeps the
+    # local path's sparsity)
+    starts = [(0, 6, 10, 14), (2, 4, 1, 6)] if not large else [(10, 50, 90, 130), (25, 65, 105, 136)]
+    for n, s_run, s_gap in zip(range(13, 17), *starts):
+        _add_landmark(pb, range(s_run, s_run + n), rng, 30.0)
+        _add_landmark(pb, s_gap + np.sort(rng.choice(n + 8, n, replace=False)), rng, 35.0)
+    for n, s in ((8, 3), (9, 17)):                      # past the 8 candidates the block-gather kernel looks up without a loop
+        _add_landmark(pb, range(s, s + n), rng, 25.0)
+    return Case("long_tracks", pb)
+
+
+CASES = {f.__name__: f for f in (scattered_fixed, isolated_cameras, sparse_landmarks, wide_landmarks, two_components, measurement_forms,
+                                 long_tracks)}
 
 
 def build(name: str, large: bool = False) -> Case:
     c = CASES[name](large)
     check(c.pb)
     return c
+
+
+# ---- numeric-edge graphs of the elimination tests (not in CASES: their conditioning would loosen the trajectory bars of the parity
+# tests); each returns (problem, Huber delta) -----------------------------------------------------------------------------------------------
+def _add_at(pb, cams, p, rng):
+    """A free landmark at world point p (estimate and truth), observed by `cams` through their INITIAL poses with one pixel of noise."""
+    cams = np.asarray(sorted(cams), np.int32)
+    T = pb.cam_pose_wc
+    R = synth._quat_to_R(T[cams, :4] / np.linalg.norm(T[cams, :4], axis=1, keepdims=True))
+    pc = np.einsum("nji,nj->ni", R, p[None] - T[cams, 4:])
+    assert (pc[:, 2] > 0).all()
+    uv = pc[:, :2] / pc[:, 2:3] + PIXEL * rng.standard_normal((cams.shape[0], 2))
+    j = pb.n_points
+    pb.points = np.ascontiguousarray(np.vstack([pb.points, p])); pb.gt_points = np.vstack([pb.gt_points, p])
+    pb.point_free = np.append(pb.point_free, np.uint8(1))
+    pb.obs_cam = np.ascontiguousarray(np.append(pb.obs_cam, cams))
+    pb.obs_point = np.ascontiguousarray(np.append(pb.obs_point, np.full(cams.shape[0], j, np.int32)))
+    pb.obs_xyz = np.ascontiguousarray(np.vstack([pb.obs_xyz, np.c_[uv, np.ones(cams.shape[0])]]))
+    return j
+
+
+def _ahead(pb, c, v):
+    """World point v = (x, y, z) in the initial frame of camera c."""
+    T = pb.cam_pose_wc[c]
+    return synth._quat_to_R((T[:4] / np.linalg.norm(T[:4]))[None])[0] @ np.asarray(v, float) + T[4:]
+
+
+def far_landmarks():
+    pb = synth.synth_ba(30, 300, obs_per_point=4, n_fixed=2, seed=181)
+    rng = np.random.default_rng(1)
+    for k, depth in enumerate((1e3, 3e3, 1e4, 3e4, 1e5)):
+        for s in (2 + 5 * k, 4 + 5 * k):
+            _add_at(pb, range(s, s + 4), _ahead(pb, s + 2, [rng.uniform(-0.2, 0.2) * depth, rng.uniform(-0.1, 0.1) * depth, depth]), rng)
+    return pb, 0.01
+
+
+def near_landmarks():
+    pb = synth.synth_ba(30, 300, obs_per_point=4, n_fixed=2, seed=182)
+    rng = np.random.default_rng(2)
+    for c in range(3, 29, 3):
+        _add_at(pb, [c - 1, c], _ahead(pb, c, [0.004, -0.003, 0.05]), rng)
+    return pb, 0.01
+
+
+def narrow_baseline():
+    pb = synth.synth_ba(30, 300, obs_per_point=4, n_fixed=2, seed=183)
+    rng = np.random.default_rng(3)
+    for c in range(2, 28, 2):
+        base = np.linalg.norm(pb.cam_pose_wc[c + 1, 4:] - pb.cam_pose_wc[c, 4:])
+        _add_at(pb, [c, c + 1], _ahead(pb, c, [0.0, 0.0, 1e4 * base]), rng)
+    return pb, 0.01
+
+
+def huber_linear():
+    pb = synth.synth_ba(30, 500, obs_per_point=4, n_fixed=2, seed=184)
+    Rwc = synth._quat_to_R(pb.cam_pose_wc[:, :4])
+    q = np.einsum("nji,nj->ni", Rwc[pb.obs_cam], pb.points[pb.obs_point] - pb.cam_pose_wc[pb.obs_cam, 4:])
+    e = np.linalg.norm(q[:, :2] / q[:, 2:3] - pb.obs_xyz[:, :2], axis=1)
+    return pb, float(np.quantile(e, 0.2))
+
+
+def fixed_only_cameras():
+    pb = synth.synth_ba(30, 500, obs_per_point=4, n_fixed=2, seed=185)
+    for c in (9, 21):
+        pb.point_free[np.unique(pb.obs_point[pb.obs_cam == c])] = 0
+    return pb, 0.01
+
+
+INDEFINITE = (10, 50, 90, 130)
+
+
+def indefinite_info():
+    """Every edge of landmarks INDEFINITE carries the indefinite information [[1, 3], [3, 1]] (eigenvalues 4 and -2): their V, damped
+    at a small lambda, is far from positive definite, so the device's Cholesky fails and damped_vinv zeroes their inverse."""
+    pb = synth.synth_ba(30, 300, obs_per_point=4, n_fixed=2, seed=186)
+    info = np.tile(np.array([1.0, 0.0, 0.0, 1.0]), (pb.n_obs, 1))
+    info[np.isin(pb.obs_point, INDEFINITE)] = [1.0, 3.0, 3.0, 1.0]
+    pb.obs_info = np.ascontiguousarray(info)
+    return pb, 0.01
+
+
+def rejected_step():
+    """20 degree rotation noise and no Huber kernel: at lambda 1e-8 the first Gauss-Newton step overshoots and is rejected (the oracle
+    rejects it too), with a camera step far from zero; at lambda 1e-4 it is accepted."""
+    return synth.synth_ba(30, 500, obs_per_point=4, n_fixed=2, seed=191, pose_sigma_deg=20.0, pose_sigma_t=0.5), 0.0
+
+
+EDGES = {f.__name__: f for f in (far_landmarks, near_landmarks, narrow_baseline, huber_linear, fixed_only_cameras, indefinite_info)}
+
 
 
 # ---- boundary graphs: one just under / over each host-side threshold ------------------------------------------------------------------
