@@ -1515,29 +1515,25 @@ int gb_ba_graph_destroy(gb_ctx* ctx, gb_ba_graph* g) {
       gb_set_error(ctx, "gb_ba_graph_destroy: a solve of this graph is still waiting for the device on another thread");
       return GB_ERR_INVALID;
     }
-    if (!g->from_arena || g->sw_alloc || g->d.prof) cudaStreamSynchronize(ctx->stream);
+    if (g->slab || g->sw_alloc || g->d.prof) cudaStreamSynchronize(ctx->stream);
   }
   ba_sweep_plan_drop(g);
   cudaFree(g->d.prof);
   if (g->h_sc) cudaFreeHost(g->h_sc);
   for (cudaEvent_t ev : {g->ev_s, g->ev_e, g->ev_done})
     if (ev) cudaEventDestroy(ev);
-  if (g->from_arena) {
-    if (ctx) ctx->ba_arena_busy = false;
-  } else {
-    cudaFree(g->slab);
-  }
+  cudaFree(g->slab);
   delete g;
   return GB_OK;
 }
 
 int gb_ba_graph_create(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out) {
-  return ba_graph_create_impl(ctx, pb, out, false, 0, 1);
+  return ba_graph_create_impl(ctx, pb, out, BaPlace::own, 0, 1);
 }
 
 // a BundleGraph with pose-graph terms (se3Graph / gpsGraph, Optimizer.h:163-168); `edges` may be NULL
 int gb_ba_graph_create_ex(gb_ctx* ctx, const gb_ba_problem* pb, const gb_pose_edges* edges, gb_ba_graph** out) {
-  return ba_graph_create_impl(ctx, pb, out, false, 0, 1, edges);
+  return ba_graph_create_impl(ctx, pb, out, BaPlace::own, 0, 1, edges);
 }
 
 }  // extern "C"
@@ -1666,7 +1662,11 @@ extern "C" GB_API int gb_dbg_ba_shard_bounds(int n_points, int n_obs, const int3
   return GB_OK;
 }
 
-int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out, bool use_arena, int shard_rank, int shard_world,
+// places a graph in the topology cache's buffer (BaPlace::cache; defined with the cache, below)
+template <typename F>
+static int ba_cache_slab(gb_ctx* ctx, F&& layout);
+
+int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out, BaPlace place, int shard_rank, int shard_world,
                          const gb_pose_edges* pose_edges) {
   if (!ctx || !out) return GB_ERR_INVALID;
   *out = nullptr;
@@ -1677,7 +1677,6 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   GB_CHECK(ba_pose_validate(ctx, pb, pose_edges));
   const int npe = pose_edges ? pose_edges->n_se3 + pose_edges->n_gps : 0;
   if (npe > 0 && shard_world > 1) { gb_set_error(ctx, "gb_ba: pose-graph terms are not sharded (single-GPU solve)"); return GB_ERR_INVALID; }
-  if (use_arena && ctx->ba_cached) ba_cache_drop(ctx);  // (another host-buffer call wants the arena the cached graph lives in)
   tr.stamp("validate");
   const int nc = pb->n_cams, np_full = pb->n_points, no_full = pb->n_obs;
   gb_ba_graph* g = new gb_ba_graph();
@@ -1872,33 +1871,17 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
     }
     if (npe > 0) sl.take(&d.pe_H, pose.rec_doubles);
   };
-  Slab measure;
-  layout(measure);
-  const size_t need = measure.off + 256;
-  g->from_arena = use_arena && !ctx->ba_arena_busy;
-  if (g->from_arena && need > ctx->ba_arena_cap) {  // grow the arena (with a quarter to spare: windows grow a little at a time)
-    GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->ba_arena);
-    ctx->ba_arena = nullptr;
-    ctx->ba_arena_cap = 0;
-  }
-  void** dst = g->from_arena ? &ctx->ba_arena : (void**)&g->slab;
-  if (!*dst) {
-    const size_t bytes = g->from_arena ? need + need / 4 : need;
-    GB_CUDA(ctx, cudaMalloc(dst, bytes));
-    if (g->from_arena) ctx->ba_arena_cap = bytes;
-  }
-  if (g->from_arena) {
-    g->slab = (uint8_t*)ctx->ba_arena;
-    ctx->ba_arena_busy = true;
-  }
-  g->slab_bytes = need;
+  Slab placed;  // the layout as placed: its base and the size of its blob
+  auto place_layout = [&](Slab& sl) { layout(sl); placed = sl; };
+  if (place == BaPlace::own) GB_CHECK(gb_slab_alloc(ctx, (void**)&g->slab, place_layout));
+  else if (place == BaPlace::cache) GB_CHECK(ba_cache_slab(ctx, place_layout));
+  else GB_CHECK(gb_scratch_slab(ctx, place_layout));
   tr.stamp("slab");
 
   // ---- one pinned blob, one H2D ------------------------------------------------------------------------------------------
   uint8_t* h_blob;
-  GB_CHECK(gb_stage_take(ctx, {{&h_blob, measure.blob}}));
-  Slab real{g->slab, h_blob};
+  GB_CHECK(gb_stage_take(ctx, {{&h_blob, placed.blob}}));
+  Slab real{placed.base, h_blob};
   layout(real);
   ba_fill_measurements(pb, order, cam_perm, real.host(d.o_uv), real.host(d.c_uv), d.has_info ? real.host(d.o_info) : nullptr);
   g->sorted_to_orig.swap(order);
@@ -1917,8 +1900,8 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   GB_CHECK(gb_ba_graph_reset(ctx, g));
   tr.stamp("enqueue H2D + prepare");
   // the pinned blob is reused by the next outermost call on this ctx: a graph handed to the caller must have consumed it; the
-  // one-shot host-buffer paths (gb_ba_solve / gb_ba_pnp) synchronise in their own finish + download before they return
-  if (!use_arena) GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  // host-buffer paths (gb_ba_solve / gb_ba_solve_posegraph / gb_ba_pnp) synchronise in their own finish + download before they return
+  if (place == BaPlace::own) GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   tr.stamp("sync");
   guard.ok = true;
   *out = g;
@@ -2364,10 +2347,15 @@ int gb_ba_graph_download(gb_ctx* ctx, gb_ba_graph* g, double* cam_pose_wc, doubl
 
 // ---- host-buffer solve with a topology cache ------------------------------------------------------------------------------------
 // A SLAM's mapping thread re-solves a sliding window whose graph changes by one keyframe now and then but mostly only in its
-// ESTIMATES.  gb_ba_solve keeps the graph of its previous call (and the arena it lives in); when the next problem has the same
-// cameras / landmarks / edges / masks (exact memcmp of the index arrays, ~10 us at the benchmark window) only poses, points and
-// measurements are uploaded -- the ~165 us of sorting, covisibility structure, plans and blob fill are skipped.
-struct BaCacheKey {
+// ESTIMATES.  gb_ba_solve keeps the graph of its previous call in a buffer of the cache's own (BaPlace::cache), which no other call
+// on the ctx touches; when the next problem has the same cameras / landmarks / edges / masks (exact memcmp of the index arrays,
+// ~10 us at the benchmark window) only poses, points and measurements are uploaded -- the ~165 us of sorting, covisibility
+// structure, plans and blob fill are skipped.  A problem that misses the cache replaces the kept graph.
+struct BaCache {
+  gb_ba_graph* g = nullptr;  // the kept graph, if any
+  uint8_t* buf = nullptr;    // the grow-only device buffer it lives in
+  size_t cap = 0;
+  // the topology of g
   int nc = 0, np = 0, no = 0;
   bool has_dof = false, has_pf = false, has_info = false;
   std::vector<int32_t> oc, op;
@@ -2389,11 +2377,33 @@ struct BaCacheKey {
   }
 };
 
-void ba_cache_drop(gb_ctx* ctx) {
-  if (!ctx) return;
-  if (ctx->ba_cached) { gb_ba_graph_destroy(ctx, ctx->ba_cached); ctx->ba_cached = nullptr; }
-  delete (BaCacheKey*)ctx->ba_cache_key;
-  ctx->ba_cache_key = nullptr;
+// BaPlace::cache, as gb_slab_alloc: places `layout` in the cache's buffer, which keeps no graph then.  The buffer grows with a
+// quarter to spare (sliding windows grow a little at a time), after a synchronisation: nothing may be in flight from the old one.
+template <typename F>
+static int ba_cache_slab(gb_ctx* ctx, F&& layout) {
+  if (!ctx->ba_cache) ctx->ba_cache = new BaCache();
+  BaCache& c = *ctx->ba_cache;
+  Slab sl;
+  layout(sl);
+  if (sl.off > c.cap) {
+    GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    cudaFree(c.buf);
+    c.buf = nullptr;
+    c.cap = 0;
+    GB_CUDA(ctx, cudaMalloc((void**)&c.buf, sl.off + sl.off / 4));
+    c.cap = sl.off + sl.off / 4;
+  }
+  sl = Slab{c.buf};
+  layout(sl);
+  return GB_OK;
+}
+
+void ba_cache_free(gb_ctx* ctx) {
+  if (!ctx->ba_cache) return;
+  gb_ba_graph_destroy(ctx, ctx->ba_cache->g);
+  cudaFree(ctx->ba_cache->buf);
+  delete ctx->ba_cache;
+  ctx->ba_cache = nullptr;
 }
 
 // new estimates / measurements into a cached graph of the same topology (one pinned blob, three H2D copies, no structure work)
@@ -2439,27 +2449,29 @@ extern "C" int gb_ba_solve(gb_ctx* ctx, gb_ba_problem* pb, const gb_ba_options* 
   CtxLock lk(ctx);
   BaTrace tr;
   gb_ba_graph* g = nullptr;
-  BaCacheKey* key = (BaCacheKey*)ctx->ba_cache_key;
+  BaCache* c = ctx->ba_cache;
   const bool cacheable = pb->n_obs > 0 && pb->n_obs <= (1 << 22) && pb->obs_cam && pb->obs_point && pb->obs_xyz && pb->cam_pose_wc && pb->points &&
                          !getenv("GB_BA_NO_CACHE");
-  if (cacheable && ctx->ba_cached && key && key->matches(pb)) {
-    g = ctx->ba_cached;
+  if (cacheable && c && c->g && c->matches(pb)) {
+    g = c->g;
     GB_CHECK(ba_graph_refresh(ctx, g, pb));
     tr.stamp("cached topology: refresh");
   } else {
-    ba_cache_drop(ctx);
-    GB_CHECK(ba_graph_create_impl(ctx, pb, &g, true, 0, 1));
-    if (cacheable && g->from_arena) {
-      key = new BaCacheKey();
-      key->fill(pb);
-      ctx->ba_cache_key = key;
-      ctx->ba_cached = g;
+    if (c) {
+      gb_ba_graph_destroy(ctx, c->g);
+      c->g = nullptr;
+    }
+    GB_CHECK(ba_graph_create_impl(ctx, pb, &g, cacheable ? BaPlace::cache : BaPlace::scratch, 0, 1));
+    if (cacheable) {
+      c = ctx->ba_cache;  // (made by the placement)
+      c->fill(pb);
+      c->g = g;
     }
   }
   const int rc = ba_graph_solve_impl(ctx, g, opt, res, g->d.nc > 0 ? pb->cam_pose_wc : nullptr, g->d.np > 0 ? pb->points : nullptr);
   ctx->ba_last_paths = ba_paths(g);
   tr.stamp("solve + download (one sync)");
-  if (g != ctx->ba_cached) gb_ba_graph_destroy(ctx, g);
+  if (!cacheable) gb_ba_graph_destroy(ctx, g);
   return rc;
 }
 
@@ -2469,7 +2481,7 @@ extern "C" int gb_ba_solve_posegraph(gb_ctx* ctx, gb_ba_problem* pb, const gb_po
   if (!edges || edges->n_se3 + edges->n_gps <= 0) return gb_ba_solve(ctx, pb, opt, res);
   CtxLock lk(ctx);
   gb_ba_graph* g = nullptr;
-  GB_CHECK(ba_graph_create_impl(ctx, pb, &g, false, 0, 1, edges));
+  GB_CHECK(ba_graph_create_impl(ctx, pb, &g, BaPlace::scratch, 0, 1, edges));
   const int rc = ba_graph_solve_impl(ctx, g, opt, res, g->d.nc > 0 ? pb->cam_pose_wc : nullptr, g->d.np > 0 ? pb->points : nullptr);
   gb_ba_graph_destroy(ctx, g);
   return rc;
@@ -2493,7 +2505,7 @@ int gb_ba_pnp(gb_ctx* ctx, int n, const double* xyz, const double* xy1, double* 
   pb.cam_pose_wc = pose_wc; pb.cam_dof = &d; pb.points = pts.data(); pb.point_free = pf.data();
   pb.obs_cam = oc.data(); pb.obs_point = op.data(); pb.obs_xyz = xy1; pb.obs_info = nullptr;
   gb_ba_graph* g = nullptr;
-  GB_CHECK(ba_graph_create_impl(ctx, &pb, &g, true, 0, 1));
+  GB_CHECK(ba_graph_create_impl(ctx, &pb, &g, BaPlace::scratch, 0, 1));
   int rc = ba_graph_solve_impl(ctx, g, opt, res, pose_wc, nullptr);
   ctx->ba_last_paths = ba_paths(g);
   if (rc == GB_OK && info6x6) {

@@ -249,7 +249,7 @@ int gb_comm_allreduce_sum_f64(gb_comm* c, double* d_buf, size_t n) {
 // ---- the sharded solve -----------------------------------------------------------------------------------------------------
 int gb_ba_shard_create(gb_comm* c, const gb_ba_problem* full, gb_ba_graph** out) {
   if (!c || !full || !out) return GB_ERR_INVALID;
-  return ba_graph_create_impl(c->ctx, full, out, false, c->rank, c->world);
+  return ba_graph_create_impl(c->ctx, full, out, BaPlace::own, c->rank, c->world);
 }
 
 int gb_ba_shard_range(const gb_ba_graph* g, int* lo, int* hi) {

@@ -21,9 +21,7 @@ struct BaPosePlan {  // pose-graph edges and their gather plans: BaDev::pe_* / p
 
 struct gb_ba_graph {
   BaDev d{};
-  uint8_t* slab = nullptr;  // one device allocation (or the ctx arena) holding everything below but the sweep plan
-  size_t slab_bytes = 0;
-  bool from_arena = false;
+  uint8_t* slab = nullptr;  // the device allocation of a BaPlace::own graph (else null): everything below but the sweep plan
   double *pose_init = nullptr, *pts_init = nullptr, *pose_wc_out = nullptr;
   double* buf = nullptr;     // internal [S | gt | diagU | cost | pad]
   double* d_cost = nullptr;  // internal candidate cost
@@ -73,9 +71,16 @@ struct gb_ba_graph {
 };
 
 // ---- ba.cu ------------------------------------------------------------------------------------------------------------------
+// Where a graph's slab (its uploaded blob and working set) lives, one placement per lifetime:
+//  own      a graph the caller holds (gb_ba_graph_create / _ex, gb_ba_shard_create): one allocation (gb_slab_alloc), which
+//           gb_ba_graph_destroy frees;
+//  cache    the graph gb_ba_solve keeps between calls: the topology cache's grow-only buffer, reused by the next graph it keeps;
+//  scratch  a graph that a host-buffer call creates, solves and destroys within itself (gb_ba_pnp, gb_ba_solve_posegraph, an
+//           uncached gb_ba_solve): one take of the ctx scratch (gb_scratch_slab), the call's last while the graph lives.
+enum class BaPlace { own, cache, scratch };
 // shard_world > 1: keep only the landmarks of `shard_rank` (contiguous range balanced by observation count) and their edges;
 // all cameras and the GLOBAL covisibility block structure are kept, so that every rank's reduced system has the same layout.
-int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out, bool use_arena, int shard_rank, int shard_world,
+int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out, BaPlace place, int shard_rank, int shard_world,
                          const gb_pose_edges* pose_edges = nullptr);
 // one LM iteration on the COMPACT reduced layout g->rbuf = [Sb | g~ | diag U | cost | pad] (g->rbuf_doubles doubles): sweep (if
 // needed) + Schur blocks, block-CSR PCG, back-substitution + candidate cost, LM accept / reject + install.  A non-null `comm`
@@ -117,5 +122,5 @@ bool ba_chol_plan_host(gb_ctx* ctx, int nc, const int* s_rowptr, const int* s_co
 // block-skyline Cholesky solve of the damped reduced camera system in the dense-layout `buf` (+ g->d.Sb block values) + retraction
 int ba_chol_launch(gb_ctx* ctx, gb_ba_graph* g, double* buf, bool pdl);
 
-// host-buffer solve cache (ba.cu): drop the graph gb_ba_solve kept from its previous call on this ctx
-void ba_cache_drop(gb_ctx* ctx);
+// host-buffer solve cache (ba.cu): free the graph gb_ba_solve kept on this ctx and the buffer it lives in (gb_ctx_destroy)
+void ba_cache_free(gb_ctx* ctx);

@@ -16,6 +16,7 @@
 #include "../../include/gslam_b200.h"
 
 struct OrbState;  // orb.cu
+struct BaCache;   // ba.cu
 
 // A grow-only buffer that one outermost API call on a ctx bump-allocates and CtxLock resets: the pinned staging, the device scratch.
 struct GbBump {
@@ -41,12 +42,8 @@ struct gb_ctx {
   // device state owned by subsystems
   OrbState* orb = nullptr;
   int match_last_plan[4] = {0, 0, 0, 0};  // qtiles, nsplit, chunk, stereo of the last match launch (gb_dbg_match_last_plan); 0s: none
-  void* ba_arena = nullptr;      // grow-only slab reused by the host-buffer BA entry points (no cudaMalloc per call)
-  size_t ba_arena_cap = 0;
-  bool ba_arena_busy = false;
-  gb_ba_graph* ba_cached = nullptr;  // the graph of the last gb_ba_solve, kept (with the arena) while the TOPOLOGY of the calls stays
-  void* ba_cache_key = nullptr;      // the same: a sliding window re-solved with new estimates skips sorting / structure / plans
-  int ba_last_paths = 0;             // gb_dbg_ba_paths bits of the graph the last gb_ba_solve / gb_ba_pnp solved (gb_dbg_ba_last_paths)
+  BaCache* ba_cache = nullptr;  // gb_ba_solve's topology cache: the graph it keeps between calls, in a buffer of its own
+  int ba_last_paths = 0;        // gb_dbg_ba_paths bits of the graph the last gb_ba_solve / gb_ba_pnp solved (gb_dbg_ba_last_paths)
 };
 
 struct gb_features {
@@ -89,8 +86,8 @@ struct GbBuf {
 // nested call may take again only once its caller is done with its own earlier buffers.  GB_ERR_CUDA when the staging cannot grow.
 int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs);
 // The same for the ctx's grow-only device scratch: the per-call working memory of the host-buffer entry points (their temporary feature
-// sets among it), the matcher's split partials, the staged frames and the test hooks, so that the long-lived objects they read (maps,
-// vocabularies) stay immutable after creation.  Two rules:
+// sets and one-shot BA graphs among it), the matcher's split partials, the staged frames and the test hooks, so that the long-lived
+// objects they read (maps, vocabularies) stay immutable after creation.  Two rules:
 //  * Take together.  Buffers that must be live at the same time are taken in one call: growing the scratch synchronises the stream
 //    and frees the old buffer, which kills every earlier take of the outermost call (bow_run takes the uploaded descriptors of
 //    gb_bow_transform with its word, key and output buffers; gb_match_hamming its two feature sets with the partials).
@@ -98,6 +95,11 @@ int gb_stage_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs);
 //    by the stream, so a kernel launched with programmatic dependent launch must not read or write scratch before that wait
 //    (remap_level0_kernel reads only the map's table before it, match_kernel touches nothing before it; every other kernel given
 //    scratch is a plain launch).  And since the wait covers only the kernel's predecessor, every PDL kernel waits on every path.
+//    One exception: the local-BA chain (ba_linearize_kernel .. ba_backsub_commit_kernel) reads the structure and measurements of a
+//    graph before its wait, and gb_ba_pnp, gb_ba_solve_posegraph and an uncached gb_ba_solve place their graph here.  Those bytes are
+//    written by the graph's H2D upload in the same call, ahead of a plain launch (ba_rt_kernel in gb_ba_graph_begin) that precedes the
+//    chain, so no chain kernel overlaps their previous user; and each of those calls synchronises its stream before it returns, so
+//    no later call overlaps the chain.
 int gb_scratch_take(gb_ctx* ctx, std::initializer_list<GbBuf> bufs);
 // Enqueues the copy of `rows` rows of `row_bytes` from src (pitch spitch) to device memory d_dst (pitch dpitch) on the ctx stream:
 // device to device, pinned host memory directly, pageable host memory row by row through the pinned staging (one take).

@@ -112,7 +112,7 @@ bool gb_func_setup(gb_ctx* ctx, const void* fn, int smem, bool* nonportable_clus
 }
 
 extern void gb_orb_state_free(gb_ctx* ctx);
-extern void ba_cache_drop(gb_ctx* ctx);
+extern void ba_cache_free(gb_ctx* ctx);
 
 extern "C" {
 
@@ -204,11 +204,10 @@ int gb_ctx_destroy(gb_ctx* ctx) {
   {
     CtxLock lk(ctx);
     cudaStreamSynchronize(ctx->stream);
-    ba_cache_drop(ctx);
+    ba_cache_free(ctx);
     gb_orb_state_free(ctx);
     if (ctx->stage.base) cudaFreeHost(ctx->stage.base);
     cudaFree(ctx->scratch.base);
-    cudaFree(ctx->ba_arena);
     cudaEventDestroy(ctx->ev0);
     cudaEventDestroy(ctx->ev1);
     cudaEventDestroy(ctx->evs);

@@ -406,6 +406,8 @@ int gb_pnp_ransac(gb_ctx* ctx, int n, const double* xyz, const double* xy, doubl
   gb_ba_options_default(&o);
   o.huber_delta = 0.0; o.max_iterations = 20; o.function_tolerance = 1e-12; o.lambda_init = 1e-4; o.pcg_max_iters = 50; o.pcg_tol = 1e-12;
   gb_ba_result res;
+  // gb_ba_pnp takes its graph from the scratch and its blob from the staging, and a growth of either frees every earlier take of
+  // this call: d_Rt, h_cnt and h_root are read above and not after.
   const int rc = gb_ba_pnp(ctx, c, ixyz.data(), ixy1.data(), wc, 63, nullptr, &o, &res);
   st.inliers_refined = best;
   if (rc == GB_OK) {
