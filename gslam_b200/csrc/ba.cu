@@ -1515,10 +1515,8 @@ int gb_ba_graph_destroy(gb_ctx* ctx, gb_ba_graph* g) {
       gb_set_error(ctx, "gb_ba_graph_destroy: a solve of this graph is still waiting for the device on another thread");
       return GB_ERR_INVALID;
     }
-    if (g->slab || g->sw_alloc || g->d.prof) cudaStreamSynchronize(ctx->stream);
+    if (g->slab) cudaStreamSynchronize(ctx->stream);
   }
-  ba_sweep_plan_drop(g);
-  cudaFree(g->d.prof);
   if (g->h_sc) cudaFreeHost(g->h_sc);
   for (cudaEvent_t ev : {g->ev_s, g->ev_e, g->ev_done})
     if (ev) cudaEventDestroy(ev);
@@ -1665,6 +1663,12 @@ extern "C" GB_API int gb_dbg_ba_shard_bounds(int n_points, int n_obs, const int3
 // places a graph in the topology cache's buffer (BaPlace::cache; defined with the cache, below)
 template <typename F>
 static int ba_cache_slab(gb_ctx* ctx, F&& layout);
+
+// whether the graph's sweep is ba_sweep.cu's kernel, whose item plan is cut on the host
+constexpr int kSweepLargeObs = 65536;
+static bool ba_sweep_is_large(const gb_ba_graph* g) {
+  return g->sweep_mode == 2 || (g->sweep_mode == 0 && g->d.no >= kSweepLargeObs);
+}
 
 int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out, BaPlace place, int shard_rank, int shard_world,
                          const gb_pose_edges* pose_edges) {
@@ -1815,6 +1819,12 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   std::vector<int> o_pt(no), c_pt(no);
   for (int e = 0; e < no; ++e) o_pt[e] = pb->obs_point[order[e]] - lo;
   for (int idx = 0; idx < no; ++idx) c_pt[idx] = o_pt[cam_perm[idx]];
+  std::vector<int> sw_items, sw_team_off;
+  const int sw_teams = ba_sweep_teams(ctx);
+  if (ba_sweep_is_large(g)) {
+    ba_sweep_plan_host(nc, np, d.cam_split, cam_off, pt_off, sw_teams, sw_items, sw_team_off);
+    d.sw_nteams = sw_teams; d.sw_nitems = (int)(sw_items.size() / 4);
+  }
   tr.stamp("plans");
 
   // ---- layout: one slab = [uploaded blob | working set] ----------------------------------------------------------------
@@ -1848,6 +1858,7 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
       sl.put(&d.pp_off, pose.pp_off.size(), pose.pp_off.data()); sl.put(&d.pp_ij, pose.pp_ij.size(), pose.pp_ij.data());
       sl.put(&d.pp_ent, pose.pp_ent.size(), pose.pp_ent.data());
     }
+    if (d.sw_nteams > 0) { sl.put(&d.sw_items, sw_items.size(), sw_items.data()); sl.put(&d.sw_team_off, sw_team_off.size(), sw_team_off.data()); }
     sl.take(&g->pose_init, (size_t)nc * 7); sl.take(&g->pose_wc_out, (size_t)nc * 7);
     sl.take(&d.pose, (size_t)nc * 7); sl.take(&d.pose_new, (size_t)nc * 7);
     sl.take(&d.Rt, (size_t)nc * 12); sl.take(&d.Rt_new, (size_t)nc * 12);
@@ -1870,6 +1881,9 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
       sl.take(&d.sp_stageG, (size_t)d.sp_nchunks * kChunkCams * 6);
     }
     if (npe > 0) sl.take(&d.pe_H, pose.rec_doubles);
+    // the test hooks' room: a sweep plan of any split they allow (a landmark group holds at least one landmark), the PCG's stamps
+    sl.take(&g->sw_room, 4 * ((size_t)nc * std::max(d.cam_split, 4) + np) + sw_teams + 1);
+    sl.take(&g->prof_room, 8);
   };
   Slab placed;  // the layout as placed: its base and the size of its blob
   auto place_layout = [&](Slab& sl) { layout(sl); placed = sl; };
@@ -1886,7 +1900,6 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   ba_fill_measurements(pb, order, cam_perm, real.host(d.o_uv), real.host(d.c_uv), d.has_info ? real.host(d.o_info) : nullptr);
   g->sorted_to_orig.swap(order);
   g->cam_perm_h.swap(cam_perm);
-  g->pt_off_h = pt_off; g->cam_off_h = cam_off;  // (the large-graph sweep cuts its work items from these on first use)
   tr.stamp("blob fill");
   GB_CUDA(ctx, cudaMemcpyAsync(real.base, real.h, real.blob, cudaMemcpyHostToDevice, ctx->stream));
   d.red_ticket = reinterpret_cast<unsigned int*>(d.red_part + kRedPartials);
@@ -1997,12 +2010,8 @@ static int ba_pcg_cluster(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
 
 // The residual + Jacobian sweep outside the local-BA launch chain: graphs with enough observations to fill the machine take the
 // bandwidth-tuned persistent kernel (ba_sweep.cu), small ones the latency-tuned one above.  which: 3 whole, 1 cameras, 2 landmarks.
-constexpr int kSweepLargeObs = 65536;
-static bool ba_sweep_is_large(const gb_ba_graph* g) {
-  return g->sweep_mode == 2 || (g->sweep_mode == 0 && g->d.no >= kSweepLargeObs);
-}
 static int ba_launch_sweep(gb_ctx* ctx, gb_ba_graph* g, const BaDev& d, cudaStream_t s, int which) {
-  if (ba_sweep_is_large(g)) return ba_sweep_launch(ctx, g, d, s, which);
+  if (ba_sweep_is_large(g)) return ba_sweep_launch(ctx, d, s, which);
   const int pt_blocks = (which & 2) ? gb_div_up(d.np * kLpp, kPtThreads) : 0, cam_blocks = (which & 1) ? d.nc * d.cam_split : 0;
   if (pt_blocks + cam_blocks > 0) { ba_linearize_kernel<<<pt_blocks + cam_blocks, kPtThreads, 0, s>>>(d, cam_blocks); GB_LAUNCH_CHECK(ctx); }
   return GB_OK;
@@ -2487,6 +2496,29 @@ extern "C" int gb_ba_solve_posegraph(gb_ctx* ctx, gb_ba_problem* pb, const gb_po
   return rc;
 }
 
+// Cuts the item plan of a graph that now takes the large-graph sweep into its room, after a test hook changed the split or the
+// sweep.  The hooks run outside any solve, so its synchronisations cost nothing there.
+static int ba_sweep_replan(gb_ctx* ctx, gb_ba_graph* g) {
+  BaDev& d = g->d;
+  if (!ba_sweep_is_large(g)) return GB_OK;
+  std::vector<int> cam_off(d.nc + 1), pt_off(d.np + 1), plan, team_off;
+  GB_CUDA(ctx, cudaMemcpyAsync(cam_off.data(), d.cam_off, cam_off.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(pt_off.data(), d.pt_off, pt_off.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  ba_sweep_plan_host(d.nc, d.np, d.cam_split, cam_off, pt_off, ba_sweep_teams(ctx), plan, team_off);
+  d.sw_nitems = (int)(plan.size() / 4);
+  d.sw_nteams = (int)team_off.size() - 1;
+  plan.insert(plan.end(), team_off.begin(), team_off.end());
+  int* h;
+  GB_CHECK(gb_stage_take(ctx, {{&h, plan.size() * 4}}));
+  memcpy(h, plan.data(), plan.size() * 4);
+  GB_CUDA(ctx, cudaMemcpyAsync(g->sw_room, h, plan.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  d.sw_items = g->sw_room;
+  d.sw_team_off = g->sw_room + 4 * (size_t)d.sw_nitems;
+  return GB_OK;
+}
+
 extern "C" {
 
 int gb_ba_pnp(gb_ctx* ctx, int n, const double* xyz, const double* xy1, double* pose_wc, int dof, double* info6x6,
@@ -2656,8 +2688,7 @@ GB_API int gb_dbg_ba_set_cam_split(gb_ctx* ctx, gb_ba_graph* g, int split) {
   if (!ctx || !g || split < 1 || split > 4) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   g->d.cam_split = split;
-  ba_sweep_plan_drop(g);  // (the large-graph sweep's items are cut per slice)
-  return GB_OK;
+  return ba_sweep_replan(ctx, g);  // (the large-graph sweep's items are cut per slice)
 }
 
 // one half of the sweep alone (which = 1: camera pass, 2: landmark pass, 3: both) -- timing experiments (tools/sweep_bench.py)
@@ -2675,7 +2706,7 @@ GB_API int gb_dbg_ba_set_sweep(gb_ctx* ctx, gb_ba_graph* g, int mode) {
   if (!ctx || !g || mode < 0 || mode > 2) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   g->sweep_mode = mode;
-  return GB_OK;
+  return ba_sweep_replan(ctx, g);
 }
 
 GB_API int gb_dbg_ba_pcg_cluster_size(gb_ctx* ctx, gb_ba_graph* g) { return (ctx && g) ? g->pcg_cluster : -1; }
@@ -2699,8 +2730,8 @@ GB_API int gb_dbg_ba_pcg_profile(gb_ctx* ctx, gb_ba_graph* g, long long* out8) {
   if (!ctx || !g) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   if (!g->d.prof) {
-    GB_CUDA(ctx, cudaMalloc((void**)&g->d.prof, 64));
-    GB_CUDA(ctx, cudaMemset(g->d.prof, 0, 64));
+    g->d.prof = g->prof_room;
+    GB_CUDA(ctx, cudaMemsetAsync(g->d.prof, 0, 64, ctx->stream));
     return GB_OK;
   }
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

@@ -21,7 +21,7 @@ struct BaPosePlan {  // pose-graph edges and their gather plans: BaDev::pe_* / p
 
 struct gb_ba_graph {
   BaDev d{};
-  uint8_t* slab = nullptr;  // the device allocation of a BaPlace::own graph (else null): everything below but the sweep plan
+  uint8_t* slab = nullptr;  // the device allocation of a BaPlace::own graph (else null): everything below
   double *pose_init = nullptr, *pts_init = nullptr, *pose_wc_out = nullptr;
   double* buf = nullptr;     // internal [S | gt | diagU | cost | pad]
   double* d_cost = nullptr;  // internal candidate cost
@@ -64,8 +64,10 @@ struct gb_ba_graph {
   const int* chol_plan = nullptr;
   int chol_blocks = 0;
   size_t chol_smem = 0;
-  void* sw_alloc = nullptr;      // device allocation holding the large-graph sweep's item plan (BaDev::sw_*), made on first use
-  std::vector<int> pt_off_h, cam_off_h;  // host copies of pt_off / cam_off (the sweep plan is cut from them)
+  // room in the slab for what the test hooks switch on: a re-cut large-graph sweep plan (items, then team_off) of any split they
+  // allow, and the PCG's clock stamps (BaDev::prof)
+  int* sw_room = nullptr;
+  long long* prof_room = nullptr;
   // landmark shard (multi-GPU global BA): this graph holds landmarks [shard_lo, shard_hi) of the caller's problem
   int shard_lo = 0, shard_hi = 0, shard_rank = 0, shard_world = 1;
 };
@@ -107,8 +109,8 @@ int ba_pose_cost(gb_ctx* ctx, gb_ba_graph* g, cudaStream_t s);              // c
 // the bandwidth-tuned residual + Jacobian sweep of large graphs (persistent CTAs, pose table in shared memory, bulk-copied W tiles)
 void ba_sweep_plan_host(int nc, int np, int cam_split, const std::vector<int>& cam_off, const std::vector<int>& pt_off, int n_teams,
                         std::vector<int>& items4, std::vector<int>& team_off);  // host-only: item records + per-team ranges
-void ba_sweep_plan_drop(gb_ba_graph* g);  // (cam_split changed / graph destroyed)
-int ba_sweep_launch(gb_ctx* ctx, gb_ba_graph* g, const BaDev& d, cudaStream_t s, int which /* 3 whole, 1 cameras, 2 landmarks */);
+int ba_sweep_teams(const gb_ctx* ctx);  // the plan's n_teams on this ctx's device
+int ba_sweep_launch(gb_ctx* ctx, const BaDev& d, cudaStream_t s, int which /* 3 whole, 1 cameras, 2 landmarks */);
 
 // ---- ba_pcg_bcsr.cu ---------------------------------------------------------------------------------------------------------
 // Host-only: decide whether / how the multi-CTA block-CSR PCG applies to `g` (sets pcg_bcsr and the scalar bcsr_* fields, fills

@@ -31,7 +31,7 @@ struct gb_ctx {
   cudaStream_t stream = nullptr;
   bool owns_stream = true;                    // false: `stream` belongs to another ctx (gb_ctx_create_on_stream)
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // gb_timer_*
-  cudaEvent_t evs = nullptr, eve = nullptr;   // internal (gb_ba_result.gpu_ms)
+  cudaEvent_t evs = nullptr, eve = nullptr;   // internal (gb_ba_result.gpu_ms, gb_dbg_popc_peak)
   cudaEvent_t ev_x = nullptr;                 // gb_ctx_wait_for (cross-ctx ordering)
   std::recursive_mutex mu;
   std::string err;
@@ -174,6 +174,8 @@ struct Slab {
 // Places `layout` (a callable that declares its arrays on the Slab it is given) in ONE new device allocation: runs it to measure,
 // allocates, runs it again to place the arrays there.  *base receives the allocation (cudaFree releases every array at once); the
 // uploads of its puts are the caller's.
+// Device memory is allocated in three places only: here (the one slab of a long-lived object: feature set, ORB state, remap table,
+// vocabulary, BA graph), bump_grow (the ctx scratch, ctx.cu) and ba_cache_slab (the BA topology cache's buffer, ba.cu).
 template <typename F>
 int gb_slab_alloc(gb_ctx* ctx, void** base, F&& layout) {
   Slab sl;

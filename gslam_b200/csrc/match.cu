@@ -258,25 +258,20 @@ extern "C" {
 GB_API int gb_dbg_popc_peak(gb_ctx* ctx, double* popc_per_s) {
   if (!ctx || !popc_per_s) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  unsigned int* d_out = nullptr;
-  GB_CUDA(ctx, cudaMalloc((void**)&d_out, 64));
+  unsigned int* d_out;
+  GB_CHECK(gb_scratch_take(ctx, {{&d_out, 64}}));
   const int ctas = ctx->sm_count * 8, iters = 4096;
-  cudaEvent_t e0, e1;
-  GB_CUDA(ctx, cudaEventCreate(&e0));
-  GB_CUDA(ctx, cudaEventCreate(&e1));
   float best = 1e30f;
   for (int rep = 0; rep < 4; ++rep) {  // rep 0 warms up
-    GB_CUDA(ctx, cudaEventRecord(e0, ctx->stream));
+    GB_CUDA(ctx, cudaEventRecord(ctx->evs, ctx->stream));
     popc_peak_kernel<<<ctas, 256, 0, ctx->stream>>>(d_out, iters, 12345u + rep);
     GB_LAUNCH_CHECK(ctx);
-    GB_CUDA(ctx, cudaEventRecord(e1, ctx->stream));
-    GB_CUDA(ctx, cudaEventSynchronize(e1));
+    GB_CUDA(ctx, cudaEventRecord(ctx->eve, ctx->stream));
+    GB_CUDA(ctx, cudaEventSynchronize(ctx->eve));
     float ms = 0.f;
-    GB_CUDA(ctx, cudaEventElapsedTime(&ms, e0, e1));
+    GB_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->evs, ctx->eve));
     if (rep > 0 && ms < best) best = ms;
   }
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  cudaFree(d_out);
   *popc_per_s = (double)ctas * 256.0 * iters * 16.0 / (best * 1e-3);
   return GB_OK;
 }
