@@ -601,11 +601,7 @@ __global__ void __launch_bounds__(64) ba_schur_reduce_kernel(BaDev g, double* __
   }
 }
 
-// test hook helper: scatter the block-CSR values into the dense S of `buf`
-__global__ void ba_densify_kernel(BaDev g, double* __restrict__ buf) {
-  const size_t n6 = g.n6, nS = n6 * n6;
-  for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < nS; idx += (size_t)gridDim.x * blockDim.x) buf[idx] = 0.0;
-}
+// scatter the block-CSR values into the dense S of `buf` (whose other entries ba_prepare_schur_kernel wrote)
 __global__ void ba_densify_fill_kernel(BaDev g, double* __restrict__ buf) {
   const int w = blockIdx.x * blockDim.x + threadIdx.x;
   if (w >= g.s_nnzb * 36) return;
@@ -1723,7 +1719,7 @@ int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out
   const int np = hi - lo, no = e_hi - e_lo;
   d.nc = nc; d.np = np; d.no = no; d.n6 = 6 * nc; d.has_info = pb->obs_info ? 1 : 0;
   d.vinv_in_sweep = 1;
-  d.r_gt = (size_t)d.n6 * d.n6;  // dense layout unless a launch says otherwise (ba_compact_iteration)
+  d.r_gt = (size_t)d.n6 * d.n6;  // dense layout unless a launch says otherwise (ba_compact_dev)
   g->buf_doubles = ba_buf_doubles(nc);
   // covisibility block structure of S over the WHOLE graph (every rank of a sharded solve must agree on the layout): block
   // (i,i') is structurally non-zero iff some landmark is seen by both cameras
@@ -2017,6 +2013,28 @@ static int ba_launch_sweep(gb_ctx* ctx, gb_ba_graph* g, const BaDev& d, cudaStre
   return GB_OK;
 }
 
+// Sweep + Schur complement of g's landmarks into `buf`, on the layout `d` describes (g->d: the dense one, ba_compact_dev: the
+// compact one).  `dense`: ba_prepare_schur_kernel also writes the dense S of buf.  The pose-graph terms, if any, go into U, g_c and
+// the cost terms between the two.  With the covisibility block structure at hand (<= kMaxBlockCams = 2048 cameras) the S blocks
+// are formed block by block without atomics (deterministic); without it this forms none (gb_ba_graph_reduce_local's atomic path).
+static int ba_reduce(gb_ctx* ctx, gb_ba_graph* g, const BaDev& d, double* buf, bool dense) {
+  cudaStream_t s = ctx->stream;
+  GB_CHECK(ba_launch_sweep(ctx, g, d, s, 3));
+  GB_CHECK(ba_pose_linearize(ctx, g, s));
+  const size_t work = std::max<size_t>(dense ? (size_t)d.n6 * d.n6 : 0, (size_t)d.np);
+  const int nblk = (int)std::min<size_t>(std::max<size_t>((work + 255) / 256, 1), (size_t)ctx->sm_count * 8);
+  ba_prepare_schur_kernel<<<nblk, 256, 0, s>>>(d, buf, dense ? 1 : 0); GB_LAUNCH_CHECK(ctx);
+  if (d.s_nnzb > 0 && d.nc > 0) {
+    if (d.sp_nchunks > 0) {
+      ba_schur_chunks_kernel<<<d.sp_nchunks, kChunkThreads, 0, s>>>(d); GB_LAUNCH_CHECK(ctx);
+      ba_schur_reduce_kernel<<<d.s_nupper, 64, 0, s>>>(d, buf); GB_LAUNCH_CHECK(ctx);
+    } else {
+      ba_schur_blocks_kernel<<<d.s_nupper, 128, 0, s>>>(d, buf); GB_LAUNCH_CHECK(ctx);
+    }
+  }
+  return GB_OK;
+}
+
 extern "C" {
 
 int gb_ba_graph_sweep(gb_ctx* ctx, gb_ba_graph* g, double huber_delta) {
@@ -2041,25 +2059,12 @@ int gb_ba_graph_reduce_local(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
   if (!buf) buf = g->buf;
   cudaStream_t s = ctx->stream;
   d.vinv_in_sweep = ba_sweep_is_large(g) ? 0 : 1;
-  GB_CHECK(ba_launch_sweep(ctx, g, d, s, 3));
-  GB_CHECK(ba_pose_linearize(ctx, g, s));  // (pose-graph terms, if any: into U, g_c and the cost terms before they are consumed)
-  // Schur complement.  With the covisibility block structure at hand (<= kMaxBlockCams = 2048 cameras) S is formed block by block without
-  // atomics (deterministic); the local-BA solver consumes the block-CSR directly, every other consumer (one-cluster / generic
-  // PCG, the multi-GPU all-reduce) gets it scattered into the dense layout of `buf`.
+  // The local-BA solver consumes the S blocks directly; every other consumer (one-cluster / generic PCG, the direct solver, a
+  // caller's all-reduce) gets them scattered into the dense layout of `buf`.
   const bool have_blocks = d.s_nnzb > 0 && d.nc > 0;
   const bool csr_only = have_blocks && g->pcg_sparse && buf == g->buf;
-  {
-    const size_t work = std::max<size_t>(csr_only ? 0 : (size_t)d.n6 * d.n6, (size_t)d.np);
-    const int nblk = (int)std::min<size_t>(std::max<size_t>((work + 255) / 256, 1), (size_t)ctx->sm_count * 8);
-    ba_prepare_schur_kernel<<<nblk, 256, 0, s>>>(d, buf, csr_only ? 0 : 1); GB_LAUNCH_CHECK(ctx);
-  }
+  GB_CHECK(ba_reduce(ctx, g, d, buf, !csr_only));
   if (have_blocks) {
-    if (d.sp_nchunks > 0) {
-      ba_schur_chunks_kernel<<<d.sp_nchunks, kChunkThreads, 0, s>>>(d); GB_LAUNCH_CHECK(ctx);
-      ba_schur_reduce_kernel<<<d.s_nupper, 64, 0, s>>>(d, buf); GB_LAUNCH_CHECK(ctx);
-    } else {
-      ba_schur_blocks_kernel<<<d.s_nupper, 128, 0, s>>>(d, buf); GB_LAUNCH_CHECK(ctx);
-    }
     if (!csr_only) { ba_densify_fill_kernel<<<gb_div_up(d.s_nnzb * 36, 256), 256, 0, s>>>(d, buf); GB_LAUNCH_CHECK(ctx); }
   } else if (d.no > 0 && d.nc > 0) {
     ba_schur_accum_kernel<<<gb_div_up(d.no, 128), 128, 0, s>>>(d, buf); GB_LAUNCH_CHECK(ctx);
@@ -2085,45 +2090,42 @@ static BaDev ba_compact_dev(const gb_ba_graph* g) {
   return d;
 }
 
-int ba_compact_reduce(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
-  const BaDev d = ba_compact_dev(g);
+// The candidate tail of every LM iteration off the local-BA chain, after its linear solve: back-substitution of the landmarks, the
+// candidate cost (pose-graph terms included) summed into d_cost and, with a communicator, all-reduced over the landmark shards ...
+static int ba_candidate_cost(gb_ctx* ctx, gb_ba_graph* g, const BaDev& d, double* d_cost, gb_comm* comm) {
   cudaStream_t s = ctx->stream;
-  GB_CHECK(ba_launch_sweep(ctx, g, d, s, 3));
-  {
-    const int nblk = (int)std::min<size_t>(std::max<size_t>(((size_t)d.np + 255) / 256, 1), (size_t)ctx->sm_count * 8);
-    ba_prepare_schur_kernel<<<nblk, 256, 0, s>>>(d, g->rbuf, 0); GB_LAUNCH_CHECK(ctx);
-  }
-  if (d.sp_nchunks > 0) {
-    ba_schur_chunks_kernel<<<d.sp_nchunks, kChunkThreads, 0, s>>>(d); GB_LAUNCH_CHECK(ctx);
-    ba_schur_reduce_kernel<<<d.s_nupper, 64, 0, s>>>(d, g->rbuf); GB_LAUNCH_CHECK(ctx);
-  } else {
-    ba_schur_blocks_kernel<<<d.s_nupper, 128, 0, s>>>(d, g->rbuf); GB_LAUNCH_CHECK(ctx);
-  }
+  if (d.np > 0) { ba_backsub_cost_kernel<<<gb_div_up(d.np * kLpp, 128), 128, 0, s>>>(d); GB_LAUNCH_CHECK(ctx); }
+  GB_CHECK(ba_pose_cost(ctx, g, s));
+  ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np + d.npe), kRedThreads, 0, s>>>(d, d.cost_pt_new, d.np + d.npe, d_cost); GB_LAUNCH_CHECK(ctx);
+  if (comm) GB_CHECK(gb_comm_allreduce_sum_f64(comm, d_cost, 1));
+  return GB_OK;
+}
+
+// ... then the LM decision from the cost in `buf` (at d.r_gt + 2 n6) and d_cost, with the installation of an accepted candidate
+static int ba_commit(gb_ctx* ctx, const BaDev& d, const double* buf, const double* d_cost) {
+  const int n = std::max(std::max(d.nc * 12, d.np * 3), 1);
+  ba_commit_apply_kernel<<<gb_div_up(n, 256), 256, 0, ctx->stream>>>(d, buf, d_cost); GB_LAUNCH_CHECK(ctx);
+  return GB_OK;
+}
+
+int ba_compact_reduce(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
+  GB_CHECK(ba_reduce(ctx, g, ba_compact_dev(g), g->rbuf, false));
   if (comm) GB_CHECK(gb_comm_allreduce_sum_f64(comm, g->rbuf, g->rbuf_doubles));
   return GB_OK;
 }
 
-int ba_compact_step(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
+// the second half of the iteration: block-CSR PCG, the candidate tail on the compact layout
+static int ba_compact_step(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
   const BaDev d = ba_compact_dev(g);
-  cudaStream_t s = ctx->stream;
   GB_CHECK(ba_pcg_bcsr_launch(ctx, g, g->rbuf));
-  if (d.np > 0) { ba_backsub_cost_kernel<<<gb_div_up(d.np * kLpp, 128), 128, 0, s>>>(d); GB_LAUNCH_CHECK(ctx); }
-  ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np), kRedThreads, 0, s>>>(d, d.cost_pt_new, d.np, g->d_cost); GB_LAUNCH_CHECK(ctx);
-  if (comm) GB_CHECK(gb_comm_allreduce_sum_f64(comm, g->d_cost, 1));
-  const int n = std::max(std::max(d.nc * 12, d.np * 3), 1);
-  ba_commit_apply_kernel<<<gb_div_up(n, 256), 256, 0, s>>>(d, g->rbuf, g->d_cost); GB_LAUNCH_CHECK(ctx);
-  return GB_OK;
-}
-
-int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
-  GB_CHECK(ba_compact_reduce(ctx, g, comm));
-  return ba_compact_step(ctx, g, comm);
+  GB_CHECK(ba_candidate_cost(ctx, g, d, g->d_cost, comm));
+  return ba_commit(ctx, d, g->rbuf, g->d_cost);
 }
 
 // The costs of a solve come from its LM decisions (lm_decide); one that made none still reports the cost at its input estimate as
 // both initial and final cost: a sweep, the pose-graph terms and the deterministic sum (all-reduced over the shards with a
 // communicator) into the LM scalars.
-int ba_cost_at_input(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
+static int ba_cost_at_input(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm) {
   const BaDev& d = g->d;
   cudaStream_t s = ctx->stream;
   GB_CHECK(ba_launch_sweep(ctx, g, d, s, 3));
@@ -2169,26 +2171,14 @@ static int ba_pcg_dispatch(gb_ctx* ctx, gb_ba_graph* g, double* buf) {
 int gb_ba_graph_step(gb_ctx* ctx, gb_ba_graph* g, const double* buf_in, double* d_cost) {
   if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  BaDev& d = g->d;
-  cudaStream_t s = ctx->stream;
-  double* buf = buf_in ? (double*)buf_in : g->buf;
-  if (!d_cost) d_cost = g->d_cost;
-  GB_CHECK(ba_pcg_dispatch(ctx, g, buf));
-  if (d.np > 0) { ba_backsub_cost_kernel<<<gb_div_up(d.np * kLpp, 128), 128, 0, s>>>(d); GB_LAUNCH_CHECK(ctx); }
-  GB_CHECK(ba_pose_cost(ctx, g, s));
-  ba_reduce_cost_kernel<<<ba_red_blocks(ctx, d.np + d.npe), kRedThreads, 0, s>>>(d, d.cost_pt_new, d.np + d.npe, d_cost); GB_LAUNCH_CHECK(ctx);
-  return GB_OK;
+  GB_CHECK(ba_pcg_dispatch(ctx, g, buf_in ? (double*)buf_in : g->buf));
+  return ba_candidate_cost(ctx, g, g->d, d_cost ? d_cost : g->d_cost, nullptr);
 }
 
 int gb_ba_graph_commit(gb_ctx* ctx, gb_ba_graph* g, const double* buf_in, const double* d_cost) {
   if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  BaDev& d = g->d;  // (dense layout: the cost sits at r_gt = n6 * n6)
-  const double* buf = buf_in ? buf_in : g->buf;
-  if (!d_cost) d_cost = g->d_cost;
-  const int n = std::max(std::max(d.nc * 12, d.np * 3), 1);
-  ba_commit_apply_kernel<<<gb_div_up(n, 256), 256, 0, ctx->stream>>>(d, buf, d_cost); GB_LAUNCH_CHECK(ctx);
-  return GB_OK;
+  return ba_commit(ctx, g->d, buf_in ? buf_in : g->buf, d_cost ? d_cost : g->d_cost);  // (dense layout: the cost sits at r_gt = n6 * n6)
 }
 
 static int ba_read_scalars(gb_ctx* ctx, gb_ba_graph* g, BaScalars* out) {
@@ -2215,24 +2205,17 @@ static int ba_fill_result(gb_ctx* ctx, const BaScalars& h, gb_ba_result* res) {
   return GB_OK;
 }
 
-}  // extern "C"
-
-int ba_graph_finish_impl(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm, gb_ba_result* res) {
-  BaScalars h;
-  GB_CHECK(ba_read_scalars(ctx, g, &h));
-  if (h.iterations == 0) {
-    GB_CHECK(ba_cost_at_input(ctx, g, comm));
-    GB_CHECK(ba_read_scalars(ctx, g, &h));
-  }
-  return ba_fill_result(ctx, h, res);
-}
-
-extern "C" {
-
+// (the stepwise interface's caller ran the LM iterations, so whether any made a decision is read from the scalars)
 int gb_ba_graph_finish(gb_ctx* ctx, gb_ba_graph* g, gb_ba_result* res) {
   if (!ctx || !g || !g->begun) return GB_ERR_INVALID;
   CtxLock lk(ctx);
-  return ba_graph_finish_impl(ctx, g, nullptr, res);
+  BaScalars h;
+  GB_CHECK(ba_read_scalars(ctx, g, &h));
+  if (h.iterations == 0) {
+    GB_CHECK(ba_cost_at_input(ctx, g, nullptr));
+    GB_CHECK(ba_read_scalars(ctx, g, &h));
+  }
+  return ba_fill_result(ctx, h, res);
 }
 
 // local-BA fast path (block-CSR Schur + single-CTA PCG): 4 launches per LM iteration, for graphs whose estimate fits the
@@ -2255,9 +2238,20 @@ static int ba_enqueue_download(gb_ctx* ctx, gb_ba_graph* g, double* hp, double* 
   return GB_OK;
 }
 
+}  // extern "C"
+
+// Whether g's LM iterations (and gb_dbg_ba_system) run on the compact reduced system: when the block-CSR PCG solves it and g is a
+// landmark shard (`comm`; a shard of a small graph can have pcg_sparse set too) or too large for the local-BA chain
+static bool ba_iterates_compact(const gb_ba_graph* g, const gb_comm* comm) {
+  return g->pcg_bcsr && g->opt.linear_solver == 0 && (comm || !ba_takes_local4(g));
+}
+
 // LM loop of a whole solve, then ONE synchronisation for everything the host wants back: the LM scalars and, for the one-shot
-// host-buffer paths, the final T_wc poses / points (pose_out / pts_out may be null).
-static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt, gb_ba_result* res, double* pose_out, double* pts_out) {
+// host-buffer paths, the final T_wc poses / points (pose_out / pts_out may be null).  With `comm`, g is this rank's landmark shard
+// (gb_ba_shard_solve): every rank reaches the same collectives and reads the same all-reduced scalars, so all stop together.  A
+// world-1 shard may take the direct solver (gb_ba_graph_begin refuses it at world > 1) and then iterates as gb_ba_graph_solve does.
+int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm, const gb_ba_options* opt, gb_ba_result* res, double* pose_out,
+                        double* pts_out) {
   if (!ctx || !g) return GB_ERR_INVALID;
   CtxLock lk(ctx);
   GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
@@ -2265,8 +2259,8 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   // on the graph's own pinned scalars and events: a tracking thread can then order its next frame after its match on this ctx
   // (gb_ctx_wait_for) while the mapping thread still waits for this solve, and the next solve finds that frame already handed over.
   // A second solve of g that another thread starts during that wait (g->waiting) takes the locked wait, leaving g's scalars and
-  // events to the first.
-  const bool unlocked_wait = !pose_out && !pts_out && ctx->lock_depth == 1 && !g->waiting;
+  // events to the first.  A shard's solve always waits locked.
+  const bool unlocked_wait = !comm && !pose_out && !pts_out && ctx->lock_depth == 1 && !g->waiting;
   if (unlocked_wait) {
     if (!g->h_sc) GB_CUDA(ctx, cudaMallocHost((void**)&g->h_sc, sizeof(BaScalars)));
     if (!g->ev_s) GB_CUDA(ctx, cudaEventCreate(&g->ev_s));
@@ -2276,7 +2270,7 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   cudaEvent_t ev_s = unlocked_wait ? g->ev_s : ctx->evs, ev_e = unlocked_wait ? g->ev_e : ctx->eve;
   GB_CUDA(ctx, cudaEventRecord(ev_s, ctx->stream));
   const bool poll = g->opt.function_tolerance > 0.0 || g->opt.verbose;
-  const bool local4 = ba_takes_local4(g);
+  const bool local4 = !comm && ba_takes_local4(g), compact = ba_iterates_compact(g, comm);
   for (int it = 0; it < g->opt.max_iterations; ++it) {
     if (local4) {
       BaDev& d = g->d;
@@ -2288,8 +2282,9 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
       if (g->opt.linear_solver == 1) GB_CHECK(ba_chol_launch(ctx, g, g->buf, true));
       else GB_CHECK(ba_pcg_sparse_launch(ctx, g, g->buf, true));
       GB_CUDA(ctx, gb_launch_pdl(ba_backsub_commit_kernel, dim3(gb_div_up(d.np * kLpp, kTailThreads)), dim3(kTailThreads), 0, s, d, (const double*)g->buf)); GB_LAUNCH_CHECK(ctx);
-    } else if (g->pcg_bcsr && g->opt.linear_solver == 0) {  // large graph: compact block-CSR reduced system + the persistent multi-CTA PCG
-      GB_CHECK(ba_compact_iteration(ctx, g, nullptr));
+    } else if (compact) {  // compact block-CSR reduced system + the persistent multi-CTA PCG (+ the shards' all-reduces)
+      GB_CHECK(ba_compact_reduce(ctx, g, comm));
+      GB_CHECK(ba_compact_step(ctx, g, comm));
     } else {  // the stepwise interface on the dense reduced layout
       GB_CHECK(gb_ba_graph_reduce_local(ctx, g, nullptr));
       GB_CHECK(gb_ba_graph_step(ctx, g, nullptr, nullptr));
@@ -2298,14 +2293,17 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
     if (poll) {
       BaScalars h;
       GB_CHECK(ba_read_scalars(ctx, g, &h));
-      if (g->opt.verbose)
-        fprintf(stderr, "[gb_ba] it %d cost %.12e lambda %.3e accepted %d pcg %d%s\n", it, h.cost, h.lambda, h.accepted,
+      if (g->opt.verbose && (!comm || gb_comm_rank(comm) == 0)) {
+        char tag[24] = "[gb_ba]";
+        if (comm) snprintf(tag, sizeof tag, "[gb_ba x%d]", gb_comm_world(comm));
+        fprintf(stderr, "%s it %d cost %.12e lambda %.3e accepted %d pcg %d%s\n", tag, it, h.cost, h.lambda, h.accepted,
                 h.pcg_iters, h.stop ? " stop" : "");
+      }
       if (h.stop) break;
     }
   }
   if (local4) { ba_install_pending_kernel<<<1, 1024, 0, ctx->stream>>>(g->d); GB_LAUNCH_CHECK(ctx); }
-  if (g->opt.max_iterations == 0) GB_CHECK(ba_cost_at_input(ctx, g, nullptr));
+  if (g->opt.max_iterations == 0) GB_CHECK(ba_cost_at_input(ctx, g, comm));  // (no LM decision: every iteration makes one)
   GB_CUDA(ctx, cudaEventRecord(ev_e, ctx->stream));
   BaDev& dd = g->d;
   const size_t bp = pose_out ? (size_t)dd.nc * 56 : 0, bx = pts_out ? (size_t)dd.np * 24 : 0;
@@ -2335,8 +2333,10 @@ static int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options*
   return GB_OK;
 }
 
+extern "C" {
+
 int gb_ba_graph_solve(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* opt, gb_ba_result* res) {
-  return ba_graph_solve_impl(ctx, g, opt, res, nullptr, nullptr);
+  return ba_graph_solve_impl(ctx, g, nullptr, opt, res, nullptr, nullptr);
 }
 
 int gb_ba_graph_download(gb_ctx* ctx, gb_ba_graph* g, double* cam_pose_wc, double* points) {
@@ -2477,7 +2477,7 @@ extern "C" int gb_ba_solve(gb_ctx* ctx, gb_ba_problem* pb, const gb_ba_options* 
       c->g = g;
     }
   }
-  const int rc = ba_graph_solve_impl(ctx, g, opt, res, g->d.nc > 0 ? pb->cam_pose_wc : nullptr, g->d.np > 0 ? pb->points : nullptr);
+  const int rc = ba_graph_solve_impl(ctx, g, nullptr, opt, res, g->d.nc > 0 ? pb->cam_pose_wc : nullptr, g->d.np > 0 ? pb->points : nullptr);
   ctx->ba_last_paths = ba_paths(g);
   tr.stamp("solve + download (one sync)");
   if (!cacheable) gb_ba_graph_destroy(ctx, g);
@@ -2491,7 +2491,7 @@ extern "C" int gb_ba_solve_posegraph(gb_ctx* ctx, gb_ba_problem* pb, const gb_po
   CtxLock lk(ctx);
   gb_ba_graph* g = nullptr;
   GB_CHECK(ba_graph_create_impl(ctx, pb, &g, BaPlace::scratch, 0, 1, edges));
-  const int rc = ba_graph_solve_impl(ctx, g, opt, res, g->d.nc > 0 ? pb->cam_pose_wc : nullptr, g->d.np > 0 ? pb->points : nullptr);
+  const int rc = ba_graph_solve_impl(ctx, g, nullptr, opt, res, g->d.nc > 0 ? pb->cam_pose_wc : nullptr, g->d.np > 0 ? pb->points : nullptr);
   gb_ba_graph_destroy(ctx, g);
   return rc;
 }
@@ -2519,6 +2519,21 @@ static int ba_sweep_replan(gb_ctx* ctx, gb_ba_graph* g) {
   return GB_OK;
 }
 
+int ba_download_S(gb_ctx* ctx, const gb_ba_graph* g, const double* blocks, double* S) {
+  const BaDev& d = g->d;
+  const size_t n6 = d.n6, nnzb = d.s_nnzb;
+  std::vector<double> sb(nnzb * 36);
+  std::vector<int> brow(nnzb), col(nnzb);
+  GB_CUDA(ctx, cudaMemcpyAsync(sb.data(), blocks, sb.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(brow.data(), d.s_brow, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaMemcpyAsync(col.data(), d.s_col, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  memset(S, 0, n6 * n6 * sizeof(double));
+  for (size_t blk = 0; blk < nnzb; ++blk)
+    for (int k = 0; k < 36; ++k) S[(6 * (size_t)brow[blk] + k / 6) * n6 + 6 * (size_t)col[blk] + k % 6] = sb[36 * blk + k];
+  return GB_OK;
+}
+
 extern "C" {
 
 int gb_ba_pnp(gb_ctx* ctx, int n, const double* xyz, const double* xy1, double* pose_wc, int dof, double* info6x6,
@@ -2538,7 +2553,7 @@ int gb_ba_pnp(gb_ctx* ctx, int n, const double* xyz, const double* xy1, double* 
   pb.obs_cam = oc.data(); pb.obs_point = op.data(); pb.obs_xyz = xy1; pb.obs_info = nullptr;
   gb_ba_graph* g = nullptr;
   GB_CHECK(ba_graph_create_impl(ctx, &pb, &g, BaPlace::scratch, 0, 1));
-  int rc = ba_graph_solve_impl(ctx, g, opt, res, pose_wc, nullptr);
+  int rc = ba_graph_solve_impl(ctx, g, nullptr, opt, res, pose_wc, nullptr);
   ctx->ba_last_paths = ba_paths(g);
   if (rc == GB_OK && info6x6) {
     // information of the returned pose: U at the final estimate (re-linearise once; the graph holds the final state)
@@ -2593,11 +2608,8 @@ GB_API int gb_dbg_ba_reduced(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* o
   GB_CHECK(gb_ba_graph_step(ctx, g, nullptr, nullptr));
   BaDev& d = g->d;
   const size_t n6 = d.n6;
-  if (g->pcg_sparse && d.s_nnzb > 0 && d.nc > 0) {  // the local-BA path keeps S as block-CSR: scatter it into the dense layout for inspection
-    ba_densify_kernel<<<64, 256, 0, ctx->stream>>>(d, g->buf);
-    ba_densify_fill_kernel<<<gb_div_up(d.s_nnzb * 36, 256), 256, 0, ctx->stream>>>(d, g->buf);
-  }
-  if (S) GB_CUDA(ctx, cudaMemcpyAsync(S, g->buf, n6 * n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  if (S && g->pcg_sparse && d.s_nnzb > 0 && d.nc > 0) GB_CHECK(ba_download_S(ctx, g, d.Sb, S));  // (the local-BA path keeps S as block-CSR)
+  else if (S) GB_CUDA(ctx, cudaMemcpyAsync(S, g->buf, n6 * n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
   if (gt) GB_CUDA(ctx, cudaMemcpyAsync(gt, g->buf + n6 * n6, n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
   if (dc) GB_CUDA(ctx, cudaMemcpyAsync(dc, d.x, n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
   BaScalars h;
@@ -2618,22 +2630,15 @@ GB_API int gb_dbg_ba_system(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* op
   GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
   const BaDev& d = g->d;
   const size_t n6 = d.n6, nnzb = d.s_nnzb;
-  const bool compact = !ba_takes_local4(g) && g->pcg_bcsr && g->opt.linear_solver == 0;
+  const bool compact = ba_iterates_compact(g, nullptr);
   // where S is read from: the compact buffer, the block-CSR values (the single-CTA PCG and the direct solver read only those), or
   // the dense layout (one-cluster / generic PCG, pose-graph coupling included)
   const bool dense_S = !compact && !(nnzb > 0 && (g->pcg_sparse || g->opt.linear_solver == 1));
-  const double* blocks = compact ? g->rbuf : d.Sb;
   const double* tail = compact ? g->rbuf + nnzb * 36 : g->buf + n6 * n6;
   if (compact) GB_CHECK(ba_compact_reduce(ctx, g, nullptr));
   else GB_CHECK(gb_ba_graph_reduce_local(ctx, g, nullptr));
-  std::vector<double> sb(dense_S ? 0 : nnzb * 36);
-  std::vector<int> brow(dense_S ? 0 : nnzb), col(dense_S ? 0 : nnzb);
   if (S && dense_S) GB_CUDA(ctx, cudaMemcpyAsync(S, g->buf, n6 * n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  if (S && !dense_S && nnzb > 0) {
-    GB_CUDA(ctx, cudaMemcpyAsync(sb.data(), blocks, nnzb * 36 * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    GB_CUDA(ctx, cudaMemcpyAsync(brow.data(), d.s_brow, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    GB_CUDA(ctx, cudaMemcpyAsync(col.data(), d.s_col, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  }
+  else if (S) GB_CHECK(ba_download_S(ctx, g, compact ? g->rbuf : d.Sb, S));
   if (gt) GB_CUDA(ctx, cudaMemcpyAsync(gt, tail, n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
   if (diagU) GB_CUDA(ctx, cudaMemcpyAsync(diagU, tail + n6, n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // (the solver below damps S in place on some paths)
@@ -2642,11 +2647,6 @@ GB_API int gb_dbg_ba_system(gb_ctx* ctx, gb_ba_graph* g, const gb_ba_options* op
   if (x) GB_CUDA(ctx, cudaMemcpyAsync(x, d.x, n6 * 8, cudaMemcpyDeviceToHost, ctx->stream));
   BaScalars h;
   GB_CHECK(ba_read_scalars(ctx, g, &h));
-  if (S && !dense_S) {
-    memset(S, 0, n6 * n6 * sizeof(double));
-    for (size_t blk = 0; blk < nnzb; ++blk)
-      for (int k = 0; k < 36; ++k) S[(6 * (size_t)brow[blk] + k / 6) * n6 + 6 * (size_t)col[blk] + k % 6] = sb[36 * blk + k];
-  }
   if (lambda) *lambda = h.lambda;
   if (pcg_iters) *pcg_iters = h.pcg_iters;
   return GB_OK;

@@ -271,25 +271,7 @@ int gb_ba_shard_solve(gb_comm* c, gb_ba_graph* g, const gb_ba_options* opt, gb_b
   CtxLock lk(ctx);
   if (!g->pcg_bcsr || !g->rbuf) { gb_set_error(ctx, "gb_ba_shard_solve: the graph has no block-CSR reduced system"); return GB_ERR_INVALID; }
   if (g->shard_world != c->world || g->shard_rank != c->rank) { gb_set_error(ctx, "gb_ba_shard_solve: graph / communicator mismatch"); return GB_ERR_INVALID; }
-  GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
-  GB_CUDA(ctx, cudaEventRecord(ctx->evs, ctx->stream));
-  const bool poll = g->opt.function_tolerance > 0.0 || g->opt.verbose;
-  for (int it = 0; it < g->opt.max_iterations; ++it) {
-    GB_CHECK(ba_compact_iteration(ctx, g, c));
-    if (poll) {  // every rank reads the same (reduced) scalars, so every rank stops at the same iteration
-      BaScalars h;
-      GB_CUDA(ctx, cudaMemcpyAsync(&h, g->d.sc, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
-      GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-      if (g->opt.verbose && c->rank == 0)
-        fprintf(stderr, "[gb_ba x%d] it %d cost %.12e lambda %.3e accepted %d pcg %d%s\n", c->world, it, h.cost, h.lambda, h.accepted, h.pcg_iters,
-                h.stop ? " stop" : "");
-      if (h.stop) break;
-    }
-  }
-  GB_CUDA(ctx, cudaEventRecord(ctx->eve, ctx->stream));
-  GB_CHECK(ba_graph_finish_impl(ctx, g, c, res));
-  if (res) GB_CUDA(ctx, cudaEventElapsedTime(&res->gpu_ms, ctx->evs, ctx->eve));
-  return GB_OK;
+  return ba_graph_solve_impl(ctx, g, c, opt, res, nullptr, nullptr);
 }
 
 // One process, N GPUs: shard `pb` over the communicators' devices (one host thread per device), solve, write every camera
@@ -371,23 +353,13 @@ GB_API int gb_dbg_ba_shard_reduced(gb_comm* c, gb_ba_graph* g, const gb_ba_optio
   if (g->shard_world != c->world || g->shard_rank != c->rank) { gb_set_error(ctx, "gb_dbg_ba_shard_reduced: graph / communicator mismatch"); return GB_ERR_INVALID; }
   GB_CHECK(gb_ba_graph_begin(ctx, g, opt));
   GB_CHECK(ba_compact_reduce(ctx, g, allreduce ? c : nullptr));
-  const BaDev& d = g->d;
-  const size_t n6 = d.n6, nnzb = d.s_nnzb;
-  std::vector<double> rb(g->rbuf_doubles);
-  std::vector<int> brow(nnzb), col(nnzb);
-  GB_CUDA(ctx, cudaMemcpyAsync(rb.data(), g->rbuf, rb.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  GB_CUDA(ctx, cudaMemcpyAsync(brow.data(), d.s_brow, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  GB_CUDA(ctx, cudaMemcpyAsync(col.data(), d.s_col, nnzb * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  const size_t n6 = g->d.n6;
+  const double* tail = g->rbuf + 36 * (size_t)g->d.s_nnzb;
+  if (S) GB_CHECK(ba_download_S(ctx, g, g->rbuf, S));
+  if (gt) GB_CUDA(ctx, cudaMemcpyAsync(gt, tail, n6 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  if (diagU) GB_CUDA(ctx, cudaMemcpyAsync(diagU, tail + n6, n6 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  if (cost) GB_CUDA(ctx, cudaMemcpyAsync(cost, tail + 2 * n6, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   GB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (S) {
-    memset(S, 0, n6 * n6 * sizeof(double));
-    for (size_t blk = 0; blk < nnzb; ++blk)
-      for (int k = 0; k < 36; ++k) S[(6 * (size_t)brow[blk] + k / 6) * n6 + 6 * (size_t)col[blk] + k % 6] = rb[36 * blk + k];
-  }
-  const double* tail = rb.data() + 36 * nnzb;
-  if (gt) memcpy(gt, tail, n6 * sizeof(double));
-  if (diagU) memcpy(diagU, tail + n6, n6 * sizeof(double));
-  if (cost) *cost = tail[2 * n6];
   return GB_OK;
 }
 

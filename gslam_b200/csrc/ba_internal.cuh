@@ -84,18 +84,16 @@ enum class BaPlace { own, cache, scratch };
 // all cameras and the GLOBAL covisibility block structure are kept, so that every rank's reduced system has the same layout.
 int ba_graph_create_impl(gb_ctx* ctx, const gb_ba_problem* pb, gb_ba_graph** out, BaPlace place, int shard_rank, int shard_world,
                          const gb_pose_edges* pose_edges = nullptr);
-// one LM iteration on the COMPACT reduced layout g->rbuf = [Sb | g~ | diag U | cost | pad] (g->rbuf_doubles doubles): sweep (if
-// needed) + Schur blocks, block-CSR PCG, back-substitution + candidate cost, LM accept / reject + install.  A non-null `comm`
-// all-reduces the reduced system and the candidate cost of this landmark shard before they are used.
-int ba_compact_iteration(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
-// its two halves: ba_compact_reduce = sweep + Schur complement of this graph's landmarks into rbuf (+ the all-reduce);
-// ba_compact_step = PCG, back-substitution + candidate cost (+ its all-reduce), LM accept / reject
+// the first half of an LM iteration on the COMPACT reduced layout g->rbuf = [Sb | g~ | diag U | cost | pad] (g->rbuf_doubles
+// doubles): sweep + Schur complement of this graph's landmarks into rbuf; a non-null `comm` then all-reduces it over the shards
 int ba_compact_reduce(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
-int ba_compact_step(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
-// the cost at the current estimate into the LM scalars' initial and final cost (a solve that made no LM decision); `comm`: all-reduced
-int ba_cost_at_input(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm);
-// gb_ba_graph_finish, with the cost of a zero-iteration solve all-reduced over `comm` (every rank calls it) when non-null
-int ba_graph_finish_impl(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm, gb_ba_result* res);
+// a whole solve (gb_ba_graph_solve, the host-buffer solves, and with a non-null `comm` one rank of gb_ba_shard_solve): begin, the
+// LM iterations, one synchronisation; T_wc poses / points into pose_out / pts_out where non-null
+int ba_graph_solve_impl(gb_ctx* ctx, gb_ba_graph* g, gb_comm* comm, const gb_ba_options* opt, gb_ba_result* res, double* pose_out,
+                        double* pts_out);
+// test hooks: S (6N x 6N, dense) <- the block-CSR values `blocks` (36 per block of g's S structure, at block row s_brow and block
+// column s_col), 0.0 elsewhere; synchronises the stream
+int ba_download_S(gb_ctx* ctx, const gb_ba_graph* g, const double* blocks, double* S);
 
 // ---- ba_pose.cu -------------------------------------------------------------------------------------------------------------
 // pose-graph terms (SE3Edge / GPSEdge, Optimizer.h:127-148) on the stepwise dense-layout solver path
